@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-""" bench.py — collocation points/sec of the pydens fit step on B200 (BASELINE.json metric).
+""" bench.py — collocation points/sec of the pydens fit step on H100 (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # our arm (one process per GPU under torchrun)
     python bench.py --impl reference --gpus N --steps K ...   # the reference's CPU path (oracle port), rank 0
@@ -10,15 +10,15 @@ configs[1]: 2-D Poisson, 4-layer [10,12,15,1] tanh MLP, batch 100 000 per GPU (w
 
 Numbers in the JSON line:
   value      points/s, device-timed (CUDA events, max over ranks) over EXACTLY K steps replayed from a
-             CUDA graph; every step reads its own batch from an HBM-resident pool of distinct batches
-             (pool > L2 when K >= 160), so no step sees its input warm in L2.
+             CUDA graph; every step reads its own batch from an HBM-resident pool of at least 160 distinct
+             batches (128 MB at cfg2, well above the 50 MB L2), so no step sees its input warm in L2.
   e2e        the same metric through the public call `Solver.fit(niters=K, batch_size=B, sampler=...)`
              with HOST batches: per step one H2D copy of the batch from pinned memory and one D2H read of
              the loss, all inside the timed region.
   roofline   the fused kernel alone (CUDA events around K back-to-back launches): algorithmic bytes
              (4*total B/point) over time against the measured HBM peak — the path is FP32-FMA bound
              (SURVEY.md 8d), so `fp32` carries the meaningful fraction: algorithmic flops (6*C*M per
-             point) over time against 148 SMs x 128 lanes x 2 flop x the measured SM clock.
+             point) over time against 132 SMs x 128 lanes x 2 flop x the measured SM clock.
   cpu_baseline  oracle/autograd_port.py (the reference algorithm on PyTorch-CPU autograd) timed on this
              box's host cores on a bounded sample of the same workload.
 """
@@ -187,7 +187,7 @@ class Timed:
         self.local_n, self.offset = shard_batch(gbatch, world, rank)
         self.inv_n = 1.0 / gbatch
         bytes_per_batch = self.local_n * self.total * 4
-        # >= 160 distinct batches at cfg2 (the pool then exceeds the 126 MB L2); big batches are each > L2 already
+        # >= 160 distinct batches at cfg2 (the pool then exceeds the 50 MB L2); big batches are each > L2 already
         self.pool_n = int(max(2, min(max(K, 160), 256, pool_cap_bytes // max(bytes_per_batch, 1))))
         gen = torch.Generator(device=dev).manual_seed(1000 + rank)
         self.pool = torch.empty((self.pool_n, self.local_n, self.total), device=dev)
@@ -309,23 +309,23 @@ def roofline_blocks(t, kern_ms, step_ms, clk, peaks, workload):
     """ roofline of the fused kernel: the binding roof (FP32 FMA for the thread kernel, tensor cores for the tile
     kernel) first, the HBM fraction BASELINE.json asks for beside it. """
     info = t.info
-    hbm_peak = float(peaks.get('hbm_gbs', 6650.0))
-    peak_src = 'measured (MEASURED_PEAKS.json)' if 'hbm_gbs' in peaks else 'fallback (B200_PROFILING.md)'
+    hbm_peak = float(peaks.get('hbm_gbs', 3350.0))
+    peak_src = 'measured (MEASURED_PEAKS.json)' if 'hbm_gbs' in peaks else 'fallback (H100 SXM data sheet)'
     flops = info.flops_per_point * t.local_n
     byts = info.bytes_per_point * t.local_n
     ach_tf = flops / (kern_ms * 1e-3) / 1e12
     ach_gbs = byts / (kern_ms * 1e-3) / 1e9
-    sm_mhz = (clk or {}).get('sm_mhz') or float(peaks.get('sm_max_mhz', 1965.0))
+    sm_mhz = (clk or {}).get('sm_mhz') or float(peaks.get('sm_max_mhz', 1980.0))
     traffic = None
     try:
         traffic = json.load(open(os.path.join(ROOT, 'profiles', 'traffic.json'))).get(workload)
     except (OSError, ValueError):
         pass
     if info.tensor_core:
-        bf16 = float(peaks.get('bf16_tflops_sustained', peaks.get('bf16_tflops', 1590.0)))
+        bf16 = float(peaks.get('bf16_tflops_sustained', peaks.get('bf16_tflops', 989.0)))
         peak = bf16 / 2.0
         roof = {'bound': 'tensor', 'achieved': ach_tf, 'peak': peak, 'unit': 'TFLOP/s', 'frac': ach_tf / peak,
-                'traffic': traffic, 'kernel': 'wide_step_kernel (tcgen05 kind::tf32, 3xTF32)', 'kernel_ms': kern_ms,
+                'traffic': traffic, 'kernel': 'wide_step_kernel (mma.sync tf32, 3xTF32)', 'kernel_ms': kern_ms,
                 'share_of_step': kern_ms / step_ms, 'flops_per_point': int(info.flops_per_point),
                 'peak_source': 'dense TF32 = measured cuBLAS bf16 (sustained) / 2, ' + peak_src,
                 'note': 'achieved counts the ALGORITHMIC 6*C*M flops per point once; the tensor cores execute 3x that '
@@ -355,6 +355,9 @@ def main():
     ap_.add_argument('--no-e2e', action='store_true')
     ap_.add_argument('--no-extras', action='store_true', help='skip strong_cfg5 / other_configs')
     ap_.add_argument('--reps', type=int, default=10, help='repetitions of the K-step timed region (min/median/max)')
+    ap_.add_argument('--dump-outputs', metavar='DIR', default=None,
+                     help='after the timed steps, write what the last step computed (gradients, loss, updated '
+                          'parameters) as DIR/<name>.npy; the inputs are seeded, so runs with the same arguments compare')
     args = ap_.parse_args()
     K, W = args.steps, max(args.warmup, 3)
     rank = int(os.environ.get('RANK', '0'))
@@ -403,6 +406,8 @@ def main():
     ms_total = ms_sorted[len(ms_sorted) // 2]                       # median of the repetitions
     value = gbatch * K / (ms_total * 1e-3)
     last_loss = float(eng.out[eng.n_params].item())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, t)
 
     # ---------------- in-kernel sampling variant (the default `fit(sampler=None)` mode) ----------------
     sampled_value = None
@@ -475,7 +480,7 @@ def main():
             med = sorted(tms)[1]
             strong = {'workload': 'cfg5 wave3d, MLP [4, 64, 64, 64, 64, 1] Tanh', 'global_batch': 4000000, 'n_gpus': world,
                       'scaling': 'strong', 'steps': kk, 'ms_per_step': med / kk, 'value': 4000000 * kk / (med * 1e-3),
-                      'unit': 'points/s', 'kernel': 'tcgen05 tile kernel' if ts5.info.tensor_core else 'thread kernel',
+                      'unit': 'points/s', 'kernel': 'tensor-core tile kernel' if ts5.info.tensor_core else 'thread kernel',
                       'allreduce_check': ts5.allreduce_check(),
                       'note': 'same code at every N: the driver can form the 1->N strong-scaling ratio from these lines'}
             del ts5
@@ -520,7 +525,7 @@ def main():
                        inputs='HBM-resident pool of %d distinct batches (%.0f MB%s), one per step; '
                               'in-kernel Philox sampling variant reported as value_sampled'
                               % (t.pool_n, t.pool_n * local_n * total * 4 / 1e6,
-                                 ' > L2' if t.pool_n * local_n * total * 4 > 126e6 else ''),
+                                 ' > L2' if t.pool_n * local_n * total * 4 > 50e6 else ''),
                        cuda_graph=graphed, final_loss=last_loss,
                        optimizer_step=('torch.optim.Adam update in the tail of the step kernel (pinn_step_adam): one launch '
                                        'per step' if t.fused_adam else 'torch fused Adam kernels + pinn_record_loss'),
@@ -529,7 +534,7 @@ def main():
                        kernel='%s<NF=%d,NS=%d> %d threads/CTA x %d CTAs, %d B smem, %d regs, per-point state in %s'
                               % ('wide_step_kernel' if info.tensor_core else 'step_kernel', info.nf, info.ns,
                                  info.threads_per_cta, n_ctas, info.smem_bytes, info.regs_per_thread,
-                                 'TMEM + L2 slab' if info.tensor_core else ('smem' if info.activations_in_smem else 'gmem'))),
+                                 'smem + L2 slab' if info.tensor_core else ('smem' if info.activations_in_smem else 'gmem'))),
         'value_sampled': sampled_value,
         'gpu_launches': (1 if t.fused_adam else 2) * K,
         'clocks': clk,
@@ -548,6 +553,19 @@ def main():
         line['cpu_baseline'] = {k: cb[k] for k in ('value', 'unit', 'cores', 'kind', 'sample')}
     print(json.dumps(line), flush=True)
     _shutdown(dist, world)
+
+
+def dump_outputs(dirname, t):
+    """ The arrays the caller of the timed step receives after its last step: the gradient vector and loss the
+    step kernel wrote, and the flat parameters after the Adam update in its tail (float32, a few KB to a few MB). """
+    os.makedirs(dirname, exist_ok=True)
+    torch.cuda.synchronize()
+    eng = t.eng
+    out = eng.out.detach().cpu().numpy().astype(np.float32)
+    arrays = {'grads': out[:eng.n_params], 'loss': out[eng.n_params:eng.n_params + 1],
+              'params': t.solver.flat_params().cpu().numpy().astype(np.float32)}
+    for name, arr in arrays.items():
+        np.save(os.path.join(dirname, name + '.npy'), arr)
 
 
 def _peaks():

@@ -1,4 +1,4 @@
-""" The reference README's first example (README.md:25-60), unchanged apart from the import: on a B200 the fit
+""" The reference README's first example (README.md:25-60), unchanged apart from the import: on an H100 the fit
 runs in the fused kernel; without a GPU it falls back to the autograd path.
 
     python examples/poisson_quickstart.py            # 1500 steps of batch 100, like the README

@@ -1,5 +1,5 @@
 /*
- * pinn_b200.h — C ABI of the B200-native PINN fit-step engine.
+ * pinn_b200.h — C ABI of the H100-native PINN fit-step engine.
  *
  * This is the drop-in boundary for the ONE hot path of analysiscenter/pydens that this
  * repository replaces: the body of the training loop of `Solver.fit`
@@ -256,7 +256,7 @@ int pinn_step(const PinnPlan* plan,
 /*
  * Data-parallel runs: the all-reduce of [grads | loss] fused into the tail of the step kernel, over
  * NVLink peer memory — no NCCL call, no extra launch.  (The reference has no multi-device path; this
- * is the B200-native form of "one all-reduce of the tiny gradient buffer per step".)
+ * is the native form of "one all-reduce of the tiny gradient buffer per step".)
  *
  *   pinn_comm_create   allocates this rank's exchange buffer (cudaMalloc inside the library so that it
  *                      can be shared through CUDA IPC) and returns its 64-byte IPC handle;
@@ -410,7 +410,7 @@ typedef struct PinnPlanInfo {
     int32_t rows_per_point;           /* floats of per-point state kept between fwd/bwd  */
     int64_t flops_per_point;          /* algorithmic 6*C*M (SURVEY.md 8d)                */
     int32_t bytes_per_point;          /* algorithmic 4*(ndims+nparams)                   */
-    int32_t tensor_core;              /* 1: the tcgen05 / TMEM tile kernel for wide networks runs the step (3xTF32),
+    int32_t tensor_core;              /* 1: the tensor-core tile kernel for wide networks runs the step (3xTF32),
                                          0: the thread-per-point FP32 kernel                 */
     int32_t small_batch_points;       /* largest batch the cluster (point, unit)-parallel loop kernel takes through
                                          pinn_multi_step (8 CTAs x 128 points), 0: the network does not fit it         */

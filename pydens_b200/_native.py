@@ -110,7 +110,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise LibraryMissing('%s not found: build it with `python -c "import __graft_entry__ as g; g.build()"` '
-                           '(nvcc, sm_100a). pydens_b200 has no CPU fallback for the fit step.' % LIB_PATH)
+                           '(nvcc, sm_90a). pydens_b200 has no CPU fallback for the fit step.' % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
     for name in EXPORTS:
         if not hasattr(lib, name):

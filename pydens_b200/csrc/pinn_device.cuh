@@ -1,4 +1,4 @@
-// pinn_device.cuh — per-point math of the fused PINN fit step (sm_100a).
+// pinn_device.cuh — per-point math of the fused PINN fit step (sm_90a).
 //
 // Everything in this header is written per THREAD: one thread owns one collocation point and
 // walks the whole step for it (MLP forward carrying a Taylor jet, ansatz, residual program,
@@ -37,20 +37,13 @@ inline float2 make_float2(float x, float y) { float2 r; r.x = x; r.y = y; return
 #define PINN_BWD_UNR_WIDE 1
 #endif
 
-// Packed FP32x2 arithmetic: Blackwell's FFMA2 / FMUL2 do two fp32 operations per issued instruction
-// (the scalar operand is broadcast by the instruction itself).  The inner loops keep their accumulators
-// as pairs of neighbouring output units, which halves the FMA instruction count.
-#if defined(__CUDA_ARCH__)
-#define PINN_FFMA2(a2, s, c2) __ffma2_rn((a2), make_float2((s), (s)), (c2))
-#define PINN_FMUL2(a2, s)     __fmul2_rn((a2), make_float2((s), (s)))
-#define PINN_FFMA2V(a2, b2, c2) __ffma2_rn((a2), (b2), (c2))
-#define PINN_FMUL2V(a2, b2)     __fmul2_rn((a2), (b2))
-#else
+// Pairwise FP32 arithmetic: the inner loops keep their accumulators as pairs of neighbouring output units.
+// Hopper has no packed FP32x2 instruction, so each pair is two round-to-nearest scalar operations (the same
+// results a packed instruction would give).
 #define PINN_FFMA2(a2, s, c2) make_float2(fmaf((a2).x, (s), (c2).x), fmaf((a2).y, (s), (c2).y))
 #define PINN_FMUL2(a2, s)     make_float2((a2).x * (s), (a2).y * (s))
 #define PINN_FFMA2V(a2, b2, c2) make_float2(fmaf((a2).x, (b2).x, (c2).x), fmaf((a2).y, (b2).y, (c2).y))
 #define PINN_FMUL2V(a2, b2)     make_float2((a2).x * (b2).x, (a2).y * (b2).y)
-#endif
 
 namespace pinn {
 
@@ -866,7 +859,7 @@ __device__ __forceinline__ float warp_transpose_reduce(float (&v)[NV], int lane)
                 float send0 = up ? v[i] : v[i + s], send1 = up ? v[i + 1] : v[i + 1 + s];
                 float2 keep = make_float2(up ? v[i + s] : v[i], up ? v[i + 1 + s] : v[i + 1]);
                 float2 got = make_float2(__shfl_xor_sync(0xffffffffu, send0, s), __shfl_xor_sync(0xffffffffu, send1, s));
-                keep = __fadd2_rn(keep, got);
+                keep = make_float2(keep.x + got.x, keep.y + got.y);
                 v[i] = keep.x; v[i + 1] = keep.y;
             }
         } else {
@@ -961,7 +954,7 @@ PINN_HD void bwd_layer(const DevLayer& L, int below_act_id, const float* __restr
     const int n_cols = L.n_in + (fold_bias ? 1 : 0);
 #pragma unroll 1
     for (int m0 = 0; m0 < n_cols; m0 += JB) {
-        // neighbouring input units are kept as pairs: one FFMA2 serves two of them
+        // neighbouring input units are kept as pairs
         float2 post[JB / 2][C];
 #pragma unroll
         for (int h = 0; h < JB / 2; ++h) {

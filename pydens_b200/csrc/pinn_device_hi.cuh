@@ -1,4 +1,4 @@
-// pinn_device_hi.cuh — per-point math of the fused fit step for derivatives of order 3 and 4 (sm_100a).
+// pinn_device_hi.cuh — per-point math of the fused fit step for derivatives of order 3 and 4 (sm_90a).
 //
 // The reference's `D` nests arbitrarily (pydens/model_torch.py:174-178): D(D(D(f, x), x), x) is how a user writes
 // u_xxx (Korteweg-de Vries), four levels give u_xxxx (beams, Kuramoto-Sivashinsky).  Here every derivative direction

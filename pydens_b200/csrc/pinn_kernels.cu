@@ -1,4 +1,4 @@
-// pinn_kernels.cu — sm_100a kernels and the C ABI (include/pinn_b200.h) of the fused PINN fit step.
+// pinn_kernels.cu — sm_90a kernels and the C ABI (include/pinn_b200.h) of the fused PINN fit step.
 //
 // One launch of step_kernel does, for every collocation point of the batch, everything the
 // reference does between sampling and loss.backward() (pydens/model_torch.py:430-460):
@@ -172,7 +172,7 @@ struct PinnPlan {
     PinnSpec spec;
     DevPlan h;
     int device;
-    bool wide;                               // the tcgen05 tile kernel runs the step
+    bool wide;                               // the tensor-core tile kernel runs the step
     StepKernelFn fn_wide;
     MultiKernelFn fn_multi;                  // persistent multi-step kernel, or nullptr when it does not fit
     int multi_threads, multi_nwacc, multi_smem;
@@ -249,7 +249,7 @@ extern "C" int pinn_plan_create(const PinnSpec* s, int device, PinnPlan** out) {
     cudaDeviceProp prop;
     e = cudaGetDeviceProperties(&prop, device);
     if (e != cudaSuccess) { delete p; return fail(PINN_E_CUDA, "cudaGetDeviceProperties: %s", cudaGetErrorString(e)); }
-    if (prop.major != 10) { delete p; return fail(PINN_E_UNSUPPORTED, "device sm_%d%d: this library is built for sm_100a only", prop.major, prop.minor); }
+    if (prop.major != 9 || prop.minor != 0) { delete p; return fail(PINN_E_UNSUPPORTED, "device sm_%d%d: this library is built for sm_90a only", prop.major, prop.minor); }
     p->sm_count = prop.multiProcessorCount;
     p->smem_optin = (int)prop.sharedMemPerBlockOptin;
 
@@ -371,9 +371,9 @@ extern "C" int pinn_plan_create(const PinnSpec* s, int device, PinnPlan** out) {
         int mw = 0;
         const char* fk = getenv("PINN_FORCE_KERNEL");
         const bool eligible = order < 3 && wide_eligible(h, &mw);
-        // measured on B200: the tile kernel wins from 64-wide layers with many jet channels on (cfg5: 13.6 ms vs
-        // 15.3 ms); for 30-40-wide networks the CUDA-core kernel is several times faster (cfg4: 2.6 ms vs 9.3 ms) —
-        // per (unit, channel) operand handling costs as much as a 64-long FMA row
+        // the tile kernel wins from 64-wide layers with many jet channels on (H100 80GB HBM3 at 700 W, cfg5: 21.1 ms
+        // vs 32.3 ms per step); for narrower networks the per (unit, channel) operand handling costs as much as the
+        // FMA row it replaces, and the CUDA-core kernel keeps them
         bool want = eligible && mw >= 48 && (1 + s->nf + s->ns) >= 5;
         if (fk && !strcmp(fk, "thread")) want = false;
         if (fk && !strcmp(fk, "wide")) {
@@ -627,9 +627,8 @@ extern "C" int pinn_pipe_sync(PinnPipe* q) {
 }
 
 // PINN_PDL=1 launches the step kernels with programmatic stream serialization (the kernel itself waits for its
-// predecessor, griddepcontrol.wait, before it reads anything the predecessor wrote).  Measured on B200 at cfg2: plain
-// back-to-back launches 102.3 -> 100.9 us/step, graph-replayed steps unchanged (100.1 vs 100.7 us) — the graph already
-// has no launch gap to hide — so it stays opt-in.
+// predecessor, griddepcontrol.wait, before it reads anything the predecessor wrote).  Graph-replayed steps (what
+// `fit` runs) have no launch gap for it to hide, so it stays opt-in.
 static int launch_step(StepKernelFn fn, int grid, int threads, int smem_bytes, cudaStream_t st, const DevPlan& plan,
                        const StepArgs& a) {
     static int pdl = -1;

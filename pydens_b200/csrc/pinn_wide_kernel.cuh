@@ -1,24 +1,25 @@
-// pinn_wide_kernel.cuh — the fit step for WIDE networks (hidden widths 17..64) on Blackwell tensor cores.
+// pinn_wide_kernel.cuh — the fit step for WIDE networks (hidden widths 17..64) on Hopper tensor cores.
 //
 // The thread-per-point kernel (pinn_step_kernel.cuh) runs every matrix product of the step on CUDA cores and has
 // to keep `units x channels` floats of state per point; for a 64-wide network carrying 9 jet channels that is
 // 2 300 floats per point and it does not fit on the SM.  Here the same step (reference pydens/model_torch.py:430-460:
 // forward of ConvBlockModel :170-172 with the nested D() derivatives :174-178 carried as jet channels, ansatz
-// :107-128, MSE :448, loss.backward() :460) is organised around tcgen05.mma:
+// :107-128, MSE :448, loss.backward() :460) is organised around warp-level tensor-core MMAs (mma.sync m16n8k8 tf32):
 //
-//   * CTA tile = 128 collocation points = the 128 TMEM lanes; 256 threads: thread (p, half) owns point p and one
-//     half of the 64 hidden units, so every per-(point, unit) quantity is thread-private.
+//   * CTA tile = 128 collocation points; 512 threads: thread (p, quarter) owns point p and one quarter of the 64
+//     hidden units, so every per-(point, unit) quantity is thread-private.
 //   * Every hidden->hidden product, for every jet channel c, is one GEMM  Z_c[128 x 64] = A_c[128 x 64] . W^T
-//     with A_c written by the threads straight into TENSOR MEMORY (tcgen05.st) and read by the MMA from there
-//     (A-from-TMEM form), W staged K-major / 128B-swizzled in shared memory, fp32 accumulators in TMEM, read back
-//     with tcgen05.ld.  Operands are split hi/lo and multiplied as 3xTF32 (lo.hi + hi.lo + hi.hi): measured
-//     2.4e-7 relative error against fp64, i.e. fp32 grade — single-pass TF32 (7e-4) cannot hold the 1e-4 bar.
-//   * The reverse sweep is the same machinery: the data gradient  abar_{h-1} = delta_h . W  is again an
-//     A-from-TMEM GEMM, and EVERY reduction over points — weight gradients  Wbar = sum_p delta^T a  (M = 64 output
-//     units, N = 64 input units, K = the 128 points of the tile, both operands MN-major in shared memory, written
-//     row-per-thread), bias gradients, the first layer's and the output layer's weight gradients (small-N GEMMs
-//     against a [16 x 128] right-hand side) — runs on the tensor cores and accumulates IN TMEM across all tiles of
-//     the CTA.  No shuffles, no atomics: the accumulators are read out once at the end of the kernel.
+//     with A_c written row-per-thread into shared memory, W staged [n][k] in shared memory, and Z_c written back to
+//     shared memory, where the thread of each point reads its row.  Every warp computes a 16 x 32 block.  Operands
+//     are split hi/lo as they are loaded and multiplied as 3xTF32 (lo.hi + hi.lo + hi.hi): fp32 grade — single-pass
+//     TF32 (7e-4 relative) cannot hold the 1e-4 bar.
+//   * The reverse sweep is the same machinery: the data gradient  abar_{h-1} = delta_h . W  is again such a GEMM,
+//     and EVERY reduction over points — weight gradients  Wbar = sum_p delta^T a  (M = 64 output units, N = 64 input
+//     units, K = the 128 points of the tile, both operands read transposed from the same row-per-point buffers),
+//     bias gradients, the first layer's and the output layer's weight gradients (small-N GEMMs against a
+//     [16 x 128] right-hand side) — runs on the tensor cores.  Each accumulator block belongs to one warp, which
+//     adds a tile's product into a shared-memory accumulator that lives for the whole kernel: no shuffles, no
+//     atomics, a fixed summation order.  The accumulators are read out once at the end of the kernel.
 //   * Between the GEMMs the per-point state (a, z_d, z_dd per unit and channel) lives in a per-CTA slab of global
 //     memory that is written and re-read by the same thread (L2-resident working set), 256 B per (point, channel,
 //     level); the adjoint of a level overwrites the dead slot of the level above.
@@ -33,24 +34,29 @@
 namespace pinn {
 namespace wide {
 
-constexpr int T = 128;                 // points per tile (= TMEM lanes)
+constexpr int T = 128;                 // points per tile
 constexpr int NT_MAX = 512;            // threads per CTA (template NT = 256 or 512): thread = (point, 1/NH of the hidden units)
 constexpr int KW = 64;                 // padded hidden width
 constexpr int MAX_LAYERS = 6;          // linear layers (hidden levels H <= 5, hidden->hidden layers <= 4)
+constexpr int LDS = KW + 4;            // row stride (floats) of the [row][64] operands: conflict-free fragment loads
+constexpr int LXB = T + 4;             // row stride of the small right-hand sides [16][128 p]
 
-// ---- shared memory map (bytes; every MMA operand 1024-aligned) -------------------------------------------------
-constexpr int S_W_HI = 0;                       // layer weights as B operand [64 x 64] K-major SW128: 16 KB
-constexpr int S_W_LO = 16384;
-constexpr int S_GA_HI = 32768;                  // weight-gradient A operand: delta  [128 p][64 j] MN-major SW128/32B
-constexpr int S_GA_LO = S_GA_HI + 32768;
-constexpr int S_GB_HI = S_GA_LO + 32768;        // weight-gradient B operand: post-activation a, same layout
-constexpr int S_GB_LO = S_GB_HI + 32768;
-constexpr int S_R = S_GB_LO + 32768;            // 163840: R[64 k][128 p] running sum of the channel-0 adjoint
-constexpr int S_XB_HI = S_R + 32768;            // 196608: small right-hand sides [16 rows][128 p] K-major SW128
-constexpr int S_XB_LO = S_XB_HI + 8192;
-constexpr int S_MISC = S_XB_LO + 8192;          // 212992: biases, first-layer weights, scalars, barrier
-constexpr int MISC_FLOATS = 3072;
-constexpr int SMEM_BYTES = S_MISC + MISC_FLOATS * 4 + 1024;     // + alignment slack
+// ---- shared memory map (bytes) ---------------------------------------------------------------------------------
+constexpr int S_W = 0;                                  // layer weights as B operand [64 n][LDS]
+constexpr int S_A = S_W + KW * LDS * 4;                 // A operand [128 p][LDS]: jets (forward), delta (reverse)
+constexpr int S_GB = S_A + T * LDS * 4;                 // weight-gradient B operand: post-activation a_{h-1} [128 p][LDS]
+constexpr int S_D = S_GB + T * LDS * 4;                 // GEMM result [128 p][LDS]
+constexpr int S_X = S_D + T * LDS * 4;                  // exchange area between the threads of a point [24][128]
+constexpr int S_XB = S_X + 24 * T * 4;                  // small right-hand sides [16 rows][LXB]
+constexpr int S_WACC = S_XB + 16 * LXB * 4;             // weight gradients of the hidden->hidden layers [4][64 j][64 m]
+constexpr int S_SMALL1 = S_WACC + (MAX_LAYERS - 2) * KW * KW * 4;  // level 1: first-layer W / b gradients [64 k][16]
+constexpr int S_OUT = S_SMALL1 + KW * 16 * 4;           // output-layer weight gradient [64 k][8]
+constexpr int S_SMALLH = S_OUT + KW * 8 * 4;            // level h >= 2: bias gradient of layer h-1 [4][64 j][8]
+constexpr int S_MISC = S_SMALLH + (MAX_LAYERS - 2) * KW * 8 * 4;   // biases, first-layer weights, scalars
+constexpr int MISC_FLOATS = 1536;
+constexpr int SMEM_BYTES = S_MISC + MISC_FLOATS * 4;
+constexpr int ACC_FLOATS = (S_MISC - S_WACC) / 4;       // every accumulator, zeroed once per launch
+static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one CTA");
 
 // misc area (float offsets)
 constexpr int M_BIAS = 0;                       // [MAX_LAYERS][64]
@@ -59,113 +65,31 @@ constexpr int M_WD = M_W0 + 64 * 8;             // first layer applied to the di
 constexpr int M_WOUT = M_WD + PINN_MAX_DIRS * 64;   // output layer weights [64]
 constexpr int M_SCAL = M_WOUT + 64;                 // per warp: loss, sbar, bout, vbar[4]  (8 floats each)
 constexpr int M_END = M_SCAL + 8 * (NT_MAX / 32);
-static_assert(M_END <= MISC_FLOATS - 8, "misc area");
+static_assert(M_END <= MISC_FLOATS, "misc area");
 
-// ---- tensor memory map (columns) -------------------------------------------------------------------------------
-// Accumulators with M = 64 rows occupy lanes 0-15 of every 32-lane quarter; a second one interleaves at lanes 16-31.
-// Every point reduction is split in two K halves (points 0-63 / 64-127) issued by two different warps into the two
-// interleaved accumulators — fixed summation order, twice the issue rate — and the halves are added at read-out.
-constexpr int TM_A_HI = 0, TM_A_LO = 64;        // A operand of the current unit (lanes = points, columns = k)
-constexpr int TM_D = 128;                       // accumulator of the current unit
-constexpr int TM_SMALL1 = 192;                  // level-1 small accumulator [64 k x 16]: first-layer W / b gradients
-constexpr int TM_OUT = 208;                     // output-layer weight gradient [64 k x 8]
-constexpr int TM_SMALLH = 216;                  // level h >= 2: bias gradient of layer h-1 [64 j x 8], 8 columns each
-constexpr int TM_WACC = 256;                    // weight gradient of hidden->hidden layer li: 64 columns at 256 + 64 li
-constexpr uint32_t TM_HALF = 16u << 16;         // lane offset of the second K half
-
-__device__ __forceinline__ uint32_t k_sw128_off(int r, int k) {          // [k/32][r/8][r%8][128 B], 64 rows
-    return (uint32_t)((k >> 5) * 8192 + (r >> 3) * 1024 + (r & 7) * 128 + ((((k & 31) >> 2) ^ (r & 7)) << 4) + (k & 3) * 4);
+// Split x into a TF32 high part and a TF32 remainder (3xTF32 products).
+__device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(x));
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lo) : "f"(x - __uint_as_float(hi)));
 }
-__device__ __forceinline__ uint32_t xb_off(int n, int p) {               // 16 rows x 128 p, K-major SW128
-    return (uint32_t)((p >> 5) * 2048 + (n >> 3) * 1024 + (n & 7) * 128 + ((((p & 31) >> 2) ^ (n & 7)) << 4) + (p & 3) * 4);
-}
-// MN-major SW128/32B: [j/32][p][128 B], 32-byte chunks XOR (p % 4); returns the offset of the 32-byte chunk of j0..j0+7
-__device__ __forceinline__ uint32_t mn32_chunk_off(int j0, int p) {
-    return (uint32_t)((j0 >> 5) * 16384 + p * 128 + ((((j0 & 31) >> 3) ^ (p & 3)) << 5));
-}
-
-// Shared-memory matrix descriptor, split in its two words: the low word carries the start address (and LBO), which is
-// all that changes from one K step to the next — 32-bit adds of constants, no 64-bit arithmetic in the issue loop.
-__device__ __forceinline__ uint32_t desc_lo(uint32_t addr, uint32_t lbo_bytes) {
-    return ((addr >> 4) & 0x3fffu) | (((lbo_bytes >> 4) & 0x3fffu) << 16);
-}
-__host__ __device__ constexpr uint32_t desc_hi(uint32_t sbo_bytes, int layout_type) {
-    return ((sbo_bytes >> 4) & 0x3fffu) | (1u << 14) | ((uint32_t)(layout_type & 7) << 29);
-}
-constexpr uint32_t DH_K128 = desc_hi(1024, 2);      // K-major, 128-byte swizzle: 8-row groups 1024 B apart
-constexpr uint32_t DH_MN32 = desc_hi(512, 1);       // MN-major, 128-byte rows / 32-byte swizzle: 4-row K groups 512 B apart
-__device__ __forceinline__ uint32_t make_idesc(int M, int N, int a_mn, int b_mn) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// Both wrappers are called by ALL lanes of an issuing warp with warp-uniform arguments; elect.sync picks the lane
-// that issues.  Keeping the election inside the asm keeps the surrounding C++ uniform.
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                       uint32_t idesc, uint32_t acc) {
-    asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tmov.b64 da, {%1, %2};\n\tmov.b64 db, {%3, %4};\n\t"
-                 "setp.ne.b32 p, %6, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %5, p;\n\t}\n"
-                 :: "r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint32_t b_lo, uint32_t b_hi, uint32_t idesc, uint32_t acc) {
-    asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 db;\n\tmov.b64 db, {%2, %3};\n\t"
-                 "setp.ne.b32 p, %5, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], db, %4, p;\n\t}\n"
-                 :: "r"(d_tmem), "r"(a_tmem), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\tselp.u32 %0, 1, 0, q;\n\t}\n" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {      // one (elected) lane
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(smem_u32(bar)) : "memory");
-}
-// Wait for the MMAs committed to `bar`; a tensor-core fault must surface as a launch error, not as a hung GPU.
-// try_wait suspends the warp by itself (the waiting warps must not steal issue slots from the issuing ones).
-__device__ __forceinline__ void mma_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t done = 0, spins = 0;
-    long long t0 = 0;
-    while (!done) {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, 0x989680;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                     : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-        if (!done && (++spins & 63u) == 0u) {
-            const long long now = clock64();
-            if (t0 == 0) t0 = now;
-            else if (now - t0 > 8000000000ll) __trap();
-        }
-    }
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void proxy_fence() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float (&v)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-                 :: "r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-                    "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])),
-                    "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])) : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&v)[8]) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(taddr) : "memory");
-    tc_wait_ld();
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-
 __device__ __forceinline__ float tf32_rn(float x) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
     return __uint_as_float(r);
 }
-__device__ __forceinline__ void split8(const float (&v)[8], float (&hi)[8], float (&lo)[8]) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { hi[i] = tf32_rn(v[i]); lo[i] = v[i] - hi[i]; }
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
+// d += a . b as 3xTF32, small terms first
+__device__ __forceinline__ void mma3(float (&d)[4], const uint32_t (&ah)[4], const uint32_t (&al)[4],
+                                     uint32_t bh0, uint32_t bh1, uint32_t bl0, uint32_t bl1) {
+    mma_tf32(d, al, bh0, bh1);
+    mma_tf32(d, ah, bl0, bl1);
+    mma_tf32(d, ah, bh0, bh1);
+}
+
 // The slab block of one (level, channel) is laid out [k / 4][point][k % 4]: the 16-byte loads of a warp's 32
 // points are contiguous (4 cache lines per request instead of 32 with one 256-byte row per point).
 // `blk` points at this thread's first float4 of the block; units k0 .. k0+7 are two float4, T*4 floats apart.
@@ -179,13 +103,16 @@ __device__ __forceinline__ void st8(float* __restrict__ blk, int k0, const float
     *reinterpret_cast<float4*>(q) = make_float4(v[0], v[1], v[2], v[3]);
     *reinterpret_cast<float4*>(q + T * 4) = make_float4(v[4], v[5], v[6], v[7]);
 }
-// 8 consecutive j of row p of an MN-major operand; the two 16-byte halves go out in an order that depends on bit 2 of
-// p so that the eight lanes of a store wavefront hit eight different 16-byte bank groups
-__device__ __forceinline__ void st_mn8(uint8_t* base, int j0, int p, const float (&v)[8]) {
-    uint8_t* c = base + mn32_chunk_off(j0, p);
-    const float4 lo4 = make_float4(v[0], v[1], v[2], v[3]), hi4 = make_float4(v[4], v[5], v[6], v[7]);
-    if (p & 4) { *reinterpret_cast<float4*>(c + 16) = hi4; *reinterpret_cast<float4*>(c) = lo4; }
-    else       { *reinterpret_cast<float4*>(c) = lo4; *reinterpret_cast<float4*>(c + 16) = hi4; }
+// units k0..k0+7 of row p of a [128][LDS] shared-memory operand
+__device__ __forceinline__ void st_row8(uint8_t* base, int p, int k0, const float (&v)[8]) {
+    float* q = reinterpret_cast<float*>(base) + p * LDS + k0;
+    *reinterpret_cast<float4*>(q) = make_float4(v[0], v[1], v[2], v[3]);
+    *reinterpret_cast<float4*>(q + 4) = make_float4(v[4], v[5], v[6], v[7]);
+}
+__device__ __forceinline__ void ld_row8(const uint8_t* base, int p, int k0, float (&v)[8]) {
+    const float* q = reinterpret_cast<const float*>(base) + p * LDS + k0;
+    const float4 a = *reinterpret_cast<const float4*>(q), b = *reinterpret_cast<const float4*>(q + 4);
+    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
 }
 
 __host__ __device__ inline int rup(int x, int m) { return (x + m - 1) / m * m; }
@@ -196,73 +123,128 @@ __host__ __device__ inline size_t spill_floats_per_cta(int n_layers, int C) {
     return (size_t)(1 + upper * C) * T * KW;
 }
 
-// Stage one layer's weights as the B operand of a GEMM (hi / lo parts, K-major SW128, 64 x 64, zero padded).
+// Stage one layer's weights as the B operand of a GEMM ([n][k], zero padded to 64 x 64).
 //   forward  (transpose = false): B[n = out unit j][k = in unit m] = W[j][m]
 //   backward (transpose = true) : B[n = in unit m][k = out unit j] = W[j][m]
 __device__ __forceinline__ void stage_layer(uint8_t* smem, const float* __restrict__ params, const DevLayer& L, bool transpose) {
+    float* w_s = reinterpret_cast<float*>(smem + S_W);
     for (int i = threadIdx.x; i < KW * KW; i += blockDim.x) {
         const int n = i >> 6, k = i & 63;
         const int j = transpose ? k : n, m = transpose ? n : k;
-        const float w = (j < L.n_out && m < L.n_in) ? __ldg(params + L.w_off + j * L.n_in + m) : 0.0f;
-        const float hi = tf32_rn(w);
-        const uint32_t off = k_sw128_off(n, k);
-        *reinterpret_cast<float*>(smem + S_W_HI + off) = hi;
-        *reinterpret_cast<float*>(smem + S_W_LO + off) = w - hi;
+        w_s[n * LDS + k] = (j < L.n_out && m < L.n_in) ? __ldg(params + L.w_off + j * L.n_in + m) : 0.0f;
     }
 }
 
-struct MmaCtx {
-    uint32_t tmem;            // base address of the allocation
-    uint32_t smem_base;       // shared-memory address of the (aligned) operand area
-};
-
-// All issue_* functions run on a whole issuing warp with warp-uniform arguments (see mma_ss / mma_ts).
-// Columns [n0, n0 + nn) of  D[128 x N] = A(TMEM)[128 x K] . B(smem W)[N x K]^T  as 3xTF32, small terms first.
-__device__ __forceinline__ void issue_ts(const MmaCtx& m, int kp, int n0, int nn) {
-    if (nn <= 0) return;
-    const uint32_t idesc = make_idesc(128, nn, 0, 0);
-    const uint32_t d = m.tmem + TM_D + n0;
-    const uint32_t row_off = (uint32_t)(n0 >> 3) * 1024u;                // rows n0.. of the B operand
-    const uint32_t b_hi = desc_lo(m.smem_base + S_W_HI + row_off, 16), b_lo = desc_lo(m.smem_base + S_W_LO + row_off, 16);
-    const int ks = kp >> 3;
-    uint32_t acc = 0;
+// Fragment coordinates of mma.m16n8k8: g = row group, t = thread in group.
+// Columns [0, np) of  D[128 x np] = A[128 x kp] . B[np x kp]^T  (A, D: [128][LDS], B: [64][LDS]).
+// Work items (16-row block, 32-column half) are dealt to the warps.
+__device__ __forceinline__ void gemm_rows(const uint8_t* smem, int kp, int np, int warp, int n_warps) {
+    const float* A = reinterpret_cast<const float*>(smem + S_A);
+    const float* B = reinterpret_cast<const float*>(smem + S_W);
+    float* D = reinterpret_cast<float*>(const_cast<uint8_t*>(smem) + S_D);
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    for (int item = warp; item < 16; item += n_warps) {
+        const int r0 = (item >> 1) * 16, c0 = (item & 1) * 32;
+        if (c0 >= np) continue;
+        float acc[4][4];
 #pragma unroll
-    for (int term = 0; term < 3; ++term) {
-        const uint32_t a_col = m.tmem + ((term == 0) ? TM_A_LO : TM_A_HI);
-        const uint32_t b0 = (term == 1) ? b_lo : b_hi;
+        for (int nt = 0; nt < 4; ++nt)
 #pragma unroll
-        for (int s = 0; s < 8; ++s) {
-            if (s < ks) {
-                // K-step s: 32 bytes further inside the 128-byte swizzle atom, the next atom after four steps
-                mma_ts(d, a_col + 8 * s, b0 + (uint32_t)(((s >> 2) * 8192 + (s & 3) * 32) >> 4), DH_K128, idesc, acc);
-                acc = 1;
+            for (int i = 0; i < 4; ++i) acc[nt][i] = 0.0f;
+        for (int k0 = 0; k0 < kp; k0 += 8) {
+            const float* pa = A + (r0 + g) * LDS + k0 + t;
+            uint32_t ah[4], al[4];
+            split_tf32(pa[0], ah[0], al[0]);
+            split_tf32(pa[8 * LDS], ah[1], al[1]);
+            split_tf32(pa[4], ah[2], al[2]);
+            split_tf32(pa[8 * LDS + 4], ah[3], al[3]);
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) {
+                if (c0 + nt * 8 < np) {
+                    const float* pb = B + (c0 + nt * 8 + g) * LDS + k0 + t;
+                    uint32_t bh0, bl0, bh1, bl1;
+                    split_tf32(pb[0], bh0, bl0);
+                    split_tf32(pb[4], bh1, bl1);
+                    mma3(acc[nt], ah, al, bh0, bh1, bl0, bl1);
+                }
+            }
+        }
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+            if (c0 + nt * 8 < np) {
+                float* pd = D + (r0 + g) * LDS + c0 + nt * 8 + 2 * t;
+                *reinterpret_cast<float2*>(pd) = make_float2(acc[nt][0], acc[nt][1]);
+                *reinterpret_cast<float2*>(pd + 8 * LDS) = make_float2(acc[nt][2], acc[nt][3]);
             }
         }
     }
 }
-// K half `half` (points 64 half .. 64 half + 63) of  ACC[64 x 64] += GA^T . GB   (both MN-major [128 p][64])
-__device__ __forceinline__ void issue_wgrad(const MmaCtx& m, uint32_t d_tmem, int half) {
-    const uint32_t idesc = make_idesc(64, 64, 1, 1);
+// ACC[64 j x 64 m] (row stride 64) += GA^T . GB over the 128 points of the tile (GA = S_A, GB = S_GB, both
+// [128 p][LDS]); rows j < mrows and columns m < ncols.  Work items: 16 x 16 blocks.
+__device__ __forceinline__ void gemm_wgrad(uint8_t* smem, float* acc_s, int mrows, int ncols, int warp, int n_warps) {
+    const float* GA = reinterpret_cast<const float*>(smem + S_A);
+    const float* GB = reinterpret_cast<const float*>(smem + S_GB);
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    for (int item = warp; item < 16; item += n_warps) {
+        const int j0 = (item >> 2) * 16, m0 = (item & 3) * 16;
+        if (j0 >= mrows || m0 >= ncols) continue;
+        float acc[2][4];
 #pragma unroll
-    for (int term = 0; term < 3; ++term) {
-        const uint32_t a0 = desc_lo(m.smem_base + ((term == 0) ? S_GA_LO : S_GA_HI), 16384) + (uint32_t)(half * 8 * 64);
-        const uint32_t b0 = desc_lo(m.smem_base + ((term == 1) ? S_GB_LO : S_GB_HI), 16384) + (uint32_t)(half * 8 * 64);
+        for (int nt = 0; nt < 2; ++nt)
 #pragma unroll
-        for (int s = 0; s < 8; ++s) mma_ss(d_tmem, a0 + (uint32_t)(s * 64), DH_MN32, b0 + (uint32_t)(s * 64), DH_MN32, idesc, 1u);
+            for (int i = 0; i < 4; ++i) acc[nt][i] = 0.0f;
+#pragma unroll 2
+        for (int p0 = 0; p0 < T; p0 += 8) {
+            const float* pa = GA + (p0 + t) * LDS + j0 + g;
+            uint32_t ah[4], al[4];
+            split_tf32(pa[0], ah[0], al[0]);
+            split_tf32(pa[8], ah[1], al[1]);
+            split_tf32(pa[4 * LDS], ah[2], al[2]);
+            split_tf32(pa[4 * LDS + 8], ah[3], al[3]);
+#pragma unroll
+            for (int nt = 0; nt < 2; ++nt) {
+                const float* pb = GB + (p0 + t) * LDS + m0 + nt * 8 + g;
+                uint32_t bh0, bl0, bh1, bl1;
+                split_tf32(pb[0], bh0, bl0);
+                split_tf32(pb[4 * LDS], bh1, bl1);
+                mma3(acc[nt], ah, al, bh0, bh1, bl0, bl1);
+            }
+        }
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt) {
+            float* q = acc_s + (j0 + g) * KW + m0 + nt * 8 + 2 * t;
+            q[0] += acc[nt][0]; q[1] += acc[nt][1];
+            q[8 * KW] += acc[nt][2]; q[8 * KW + 1] += acc[nt][3];
+        }
     }
 }
-// K half `half` of  ACC[64 x n] += GA^T . XB^T   (GA MN-major [128 p][64], XB K-major [16 rows][128 p]), n = 8 or 16
-__device__ __forceinline__ void issue_small(const MmaCtx& m, uint32_t d_tmem, int n, int half) {
-    const uint32_t idesc = make_idesc(64, n, 1, 0);
-#pragma unroll
-    for (int term = 0; term < 3; ++term) {
-        const uint32_t a0 = desc_lo(m.smem_base + ((term == 0) ? S_GA_LO : S_GA_HI), 16384) + (uint32_t)(half * 8 * 64);
-        const uint32_t b0 = desc_lo(m.smem_base + ((term == 1) ? S_XB_LO : S_XB_HI), 16);
-#pragma unroll
-        for (int s = 0; s < 8; ++s) {
-            const int sg = half * 8 + s;
-            mma_ss(d_tmem, a0 + (uint32_t)(s * 64), DH_MN32, b0 + (uint32_t)(((sg >> 2) * 2048 + (sg & 3) * 32) >> 4), DH_K128, idesc, 1u);
+// ACC[64 j x n] (row stride n) += GA^T . XB^T over the tile (XB: [16 rows][LXB]), n = 8 or 16.  The work items
+// (16 x 8 blocks) are dealt from the last warp down, so that they land beside the items of gemm_wgrad.
+__device__ __forceinline__ void gemm_small(uint8_t* smem, float* acc_s, int n, int warp, int n_warps) {
+    const float* GA = reinterpret_cast<const float*>(smem + S_A);
+    const float* XB = reinterpret_cast<const float*>(smem + S_XB);
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const int n_items = 4 * (n >> 3);
+    for (int item = n_warps - 1 - warp; item < n_items; item += n_warps) {
+        const int j0 = (item & 3) * 16, r0 = (item >> 2) * 8;
+        float acc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+#pragma unroll 2
+        for (int p0 = 0; p0 < T; p0 += 8) {
+            const float* pa = GA + (p0 + t) * LDS + j0 + g;
+            uint32_t ah[4], al[4];
+            split_tf32(pa[0], ah[0], al[0]);
+            split_tf32(pa[8], ah[1], al[1]);
+            split_tf32(pa[4 * LDS], ah[2], al[2]);
+            split_tf32(pa[4 * LDS + 8], ah[3], al[3]);
+            const float* pb = XB + (r0 + g) * LXB + p0 + t;
+            uint32_t bh0, bl0, bh1, bl1;
+            split_tf32(pb[0], bh0, bl0);
+            split_tf32(pb[4], bh1, bl1);
+            mma3(acc, ah, al, bh0, bh1, bl0, bl1);
         }
+        float* q = acc_s + (j0 + g) * n + r0 + 2 * t;
+        q[0] += acc[0]; q[1] += acc[1];
+        q[8 * n] += acc[2]; q[8 * n + 1] += acc[3];
     }
 }
 
@@ -272,11 +254,8 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
     constexpr int C = 1 + NF + NS;
     constexpr int NH = NT / T;               // threads per point: each owns KW / NH hidden units
     constexpr int QN = KW / NH / 8;          // 8-unit chunks per thread
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    extern __shared__ __align__(16) uint8_t smem[];
     float* misc = reinterpret_cast<float*>(smem + S_MISC);
-    __shared__ uint32_t s_tmem;
-    __shared__ __align__(8) uint64_t s_bar;
 
     const int tid = threadIdx.x, p = tid & 127, kh = tid >> 7, warp = tid >> 5, lane = tid & 31;
     const int warp_u = __shfl_sync(0xffffffffu, tid >> 5, 0);        // the same number, provably warp-uniform
@@ -285,22 +264,11 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
 
     pdl_wait();                                    // the previous step (its parameter update) is complete and visible
     pdl_launch_dependents();
-    // ---- one-time setup: TMEM, barrier, constants --------------------------------------------------------------
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" :: "r"(smem_u32(&s_tmem)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (tid == 0) mbar_init(&s_bar, 4);                      // four issuing warps commit every MMA phase
+    // ---- one-time setup: constants, zeroed accumulators -----------------------------------------------------------
     for (int i = tid; i < MISC_FLOATS; i += NT) misc[i] = 0.0f;
-    for (int i = tid; i < 16384 / 4; i += NT) reinterpret_cast<float*>(smem + S_XB_HI)[i] = 0.0f;      // XB hi + lo
-    tc_fence_before();
+    for (int i = tid; i < 16 * LXB; i += NT) reinterpret_cast<float*>(smem + S_XB)[i] = 0.0f;
+    for (int i = tid; i < ACC_FLOATS; i += NT) reinterpret_cast<float*>(smem + S_WACC)[i] = 0.0f;
     __syncthreads();
-    tc_fence_after();
-    MmaCtx mc;
-    if (s_tmem != 0u) __trap();                              // all 512 columns are ours: the allocation starts at column 0, lane 0
-    mc.tmem = 0u; mc.smem_base = smem_u32(smem);
-    const uint32_t tm_lane = mc.tmem + ((uint32_t)((warp & 3) * 32) << 16);     // this warp's TMEM lanes
-    uint32_t phase = 0;
     {
         // biases of every layer, first-layer weights and their products with the direction vectors, output weights
         for (int l = 0; l < Ln; ++l)
@@ -314,14 +282,8 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
             misc[M_WD + d * 64 + k] = sum;
         }
         for (int k = tid; k < P.layer[H].n_in; k += NT) misc[M_WOUT + k] = __ldg(a.params + P.layer[H].w_off + k);
-        // zero the persistent accumulators (columns 192..511) of this thread's lane
-        const float z[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-        for (int c0 = TM_SMALL1 + kh * (320 / NH); c0 < TM_SMALL1 + (kh + 1) * (320 / NH); c0 += 8) tmem_st8(tm_lane + c0, z);
-        tc_wait_st();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
 
     // ---- per-thread views ----------------------------------------------------------------------------------------
     float* slab = a.spill + (size_t)blockIdx.x * spill_floats_per_cta(Ln, C);
@@ -329,8 +291,9 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
         const int b = (h == 1) ? 0 : 1 + (h - 2) * C + c;    // level 1 keeps channel 0 only
         return slab + (size_t)b * (T * KW) + p * 4;
     };
-    float* Xbuf = reinterpret_cast<float*>(smem + S_R);      // exchange area between the threads of a point
-    float* st = reinterpret_cast<float*>(smem + S_GA_HI) + p;    // ansatz / program scratch rows (stride T), GA/GB area
+    float* Xbuf = reinterpret_cast<float*>(smem + S_X);      // exchange area between the threads of a point
+    float* xb = reinterpret_cast<float*>(smem + S_XB);       // small right-hand sides [16][LXB]
+    float* st = reinterpret_cast<float*>(smem + S_A) + p;    // ansatz / program scratch rows (stride T), A/GB area
     constexpr int RS = T;
     const int kbeg = kh * (KW / NH);
 
@@ -340,24 +303,12 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
 #pragma unroll
     for (int i = 0; i < PINN_MAX_VARS; ++i) acc_vbar[i] = 0.0f;
 
-    // One MMA phase: everybody's operand writes are complete -> warps 0..3 each issue their share of the GEMMs (each
-    // accumulator belongs to exactly one warp, so the summation order is fixed) -> everybody waits for completion.
+    // One MMA phase: everybody's operand writes are complete -> every warp computes its share of the GEMMs (each
+    // accumulator block belongs to exactly one warp, so the summation order is fixed) -> the results are visible.
     auto sync_issue = [&](auto&& issue) {
-        tc_wait_st();
-        proxy_fence();
-        tc_fence_before();
         __syncthreads();
-        if (warp_u < 4) {                                    // warp-uniform branch; one elected lane issues the whole share
-            tc_fence_after();
-            if (elect_one()) {
-                issue(warp_u);
-                tc_commit(&s_bar);
-            }
-            __syncwarp();
-        }
-        mma_wait(&s_bar, phase);
-        phase ^= 1u;
-        tc_fence_after();
+        issue(warp_u);
+        __syncthreads();
     };
     // stored jet channel c (>= 1) of level h, units k0..k0+7: level 1 is not stored — its first-order jets are the
     // first layer applied to the direction vectors (the same for every point), its second-order jets vanish
@@ -397,18 +348,7 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
             }
         }
     };
-    auto put_A = [&](int k0, const float (&v)[8]) {          // A operand of the next GEMM, straight into tensor memory
-        float hi[8], lo[8];
-        split8(v, hi, lo);
-        tmem_st8(tm_lane + TM_A_HI + k0, hi);
-        tmem_st8(tm_lane + TM_A_LO + k0, lo);
-    };
-    auto put_G = [&](int base_hi, int base_lo, int k0, const float (&v)[8]) {    // row p of a weight-gradient operand
-        float hi[8], lo[8];
-        split8(v, hi, lo);
-        st_mn8(smem + base_hi, k0, p, hi);
-        st_mn8(smem + base_lo, k0, p, lo);
-    };
+    auto put_A = [&](int k0, const float (&v)[8]) { st_row8(smem + S_A, p, k0, v); };   // A operand of the next GEMM
 
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const long long pl = tile * T + p;
@@ -473,7 +413,7 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
                     for (int q = 0; q < QN; ++q) {
                         const int n0 = kbeg + q * 8;
                         float z[8];
-                        if (n0 < np) tmem_ld8(tm_lane + TM_D + n0, z);
+                        if (n0 < np) ld_row8(smem + S_D, p, n0, z);
                         else {
 #pragma unroll
                             for (int i = 0; i < 8; ++i) z[i] = 0.0f;
@@ -485,13 +425,10 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
                         st8(row(h + 1, c), n0, z);
                     }
                 } else {
-                    float z[8];
-                    tmem_ld8(tm_lane + TM_D, z);
-                    N[c] = z[0] + (c == 0 ? misc[M_BIAS + H * 64] : 0.0f);
+                    N[c] = reinterpret_cast<const float*>(smem + S_D)[p * LDS] + (c == 0 ? misc[M_BIAS + H * 64] : 0.0f);
                 }
-                tc_fence_before();
             };
-            auto gemm = [&](int w) { issue_ts(mc, kp, 16 * w, (16 * w < np) ? 16 : 0); };   // 16 output columns per issuing warp
+            auto gemm = [&](int w) { gemm_rows(smem, kp, np, w, NT / 32); };
             for (int g = 0; g <= NF; ++g) {
                 const int cy = group_y(g);
                 float stash[QN][8];
@@ -521,7 +458,7 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
         // a0h now holds the activations of the top level H
 
         // =========================== ansatz, residual, adjoint seed (one thread per point) ===========================
-        __syncthreads();                                     // the GA/GB area becomes program scratch
+        __syncthreads();                                     // the A/GB area becomes program scratch
         if (kh == 0) {
             float Nb[C];
             float* coords = st;
@@ -598,14 +535,10 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
                         if (cy >= 0) t[i] = fmaf(nby, ay[i], t[i]);
                     }
                 }
-                put_G(S_GA_HI, S_GA_LO, k0, t);
+                put_A(k0, t);
             }
-            if (kh == 0) {
-                *reinterpret_cast<float*>(smem + S_XB_HI + xb_off(0, p)) = 1.0f;
-                *reinterpret_cast<float*>(smem + S_XB_LO + xb_off(0, p)) = 0.0f;
-            }
-            sync_issue([&](int w) { if (w < 2) issue_small(mc, mc.tmem + TM_OUT + (w ? TM_HALF : 0u), 8, w); });
-            tc_fence_before();
+            if (kh == 0) xb[p] = 1.0f;
+            sync_issue([&](int w) { gemm_small(smem, reinterpret_cast<float*>(smem + S_OUT), 8, w, NT / 32); });
         }
         // rounds H..1: adjoint through the activation of level h, then (h >= 2) through the linear layer below it
         for (int h = H; h >= 1; --h) {
@@ -636,59 +569,44 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
                     ld8(row(h + 1, c), k0, v);
                 }
             };
-            // operands of channel c are in place (GA = delta, and for h >= 2 TMEM A = delta, GB = a_{h-1,c})
+            // operands of channel c are in place (A = GA = delta, and for h >= 2 GB = a_{h-1,c})
             auto run = [&](int c) {
                 const int d = (c == 0) ? -1 : ((c <= NF) ? c - 1 : c - 1 - NF);
                 if (kh == 0) {       // small right-hand side: row 0 = 1 for the value channel (bias gradient); level 1: the inputs
-                    *reinterpret_cast<float*>(smem + S_XB_HI + xb_off(0, p)) = (c == 0) ? 1.0f : 0.0f;
-                    *reinterpret_cast<float*>(smem + S_XB_LO + xb_off(0, p)) = 0.0f;
+                    xb[p] = (c == 0) ? 1.0f : 0.0f;
                     if (h == 1) {
 #pragma unroll
-                        for (int i = 0; i < PINN_MAX_DIMS; ++i) {
-                            if (i < P.total) {
-                                const float xv = (c == 0) ? Xbuf[(16 + i) * T + p] : ((c <= NF) ? P.dir_vec[d][i] : 0.0f);
-                                const float xh = tf32_rn(xv);
-                                *reinterpret_cast<float*>(smem + S_XB_HI + xb_off(1 + i, p)) = xh;
-                                *reinterpret_cast<float*>(smem + S_XB_LO + xb_off(1 + i, p)) = xv - xh;
-                            }
-                        }
+                        for (int i = 0; i < PINN_MAX_DIMS; ++i)
+                            if (i < P.total) xb[(1 + i) * LXB + p] = (c == 0) ? Xbuf[(16 + i) * T + p] : ((c <= NF) ? P.dir_vec[d][i] : 0.0f);
                     }
                 }
                 if (h >= 2) {
                     // warps 0/1: the data gradient, 32 columns each; warps 2/3: the two K halves of the weight
                     // gradient (and, on the value channel, of the bias gradient)
                     sync_issue([&](int w) {
-                        if (w < 2) issue_ts(mc, kp, 32 * w, (np - 32 * w) > 32 ? 32 : (np - 32 * w));
-                        else {
-                            const uint32_t hl = (w == 3) ? TM_HALF : 0u;
-                            issue_wgrad(mc, mc.tmem + TM_WACC + 64 * (h - 2) + hl, w - 2);
-                            if (c == 0) issue_small(mc, mc.tmem + TM_SMALLH + 8 * (h - 2) + hl, 8, w - 2);
-                        }
+                        gemm_rows(smem, kp, np, w, NT / 32);
+                        gemm_wgrad(smem, reinterpret_cast<float*>(smem + S_WACC) + (h - 2) * KW * KW, L.n_out, L.n_in, w, NT / 32);
+                        if (c == 0) gemm_small(smem, reinterpret_cast<float*>(smem + S_SMALLH) + (h - 2) * KW * 8, 8, w, NT / 32);
                     });
                     float* dst = row(h, c);                  // abar_{h-1,c} takes the dead slot of (h, c)
 #pragma unroll
                     for (int q = 0; q < QN; ++q) {
                         const int n0 = kbeg + q * 8;
                         float z[8];
-                        if (n0 < np) tmem_ld8(tm_lane + TM_D + n0, z);
+                        if (n0 < np) ld_row8(smem + S_D, p, n0, z);
                         else {
 #pragma unroll
                             for (int i = 0; i < 8; ++i) z[i] = 0.0f;
                         }
                         st8(dst, n0, z);
                     }
-                    tc_fence_before();
                 } else {                                     // level 1: only the first layer's own gradients
-                    sync_issue([&](int w) { if (w < 2) issue_small(mc, mc.tmem + TM_SMALL1 + (w ? TM_HALF : 0u), 16, w); });
-                    tc_fence_before();
+                    sync_issue([&](int w) { gemm_small(smem, reinterpret_cast<float*>(smem + S_SMALL1), 16, w, NT / 32); });
                 }
             };
             auto put_ops = [&](int k0, const float (&delta)[8], const float (&below)[8]) {
-                put_G(S_GA_HI, S_GA_LO, k0, delta);
-                if (h >= 2) {
-                    put_A(k0, delta);
-                    put_G(S_GB_HI, S_GB_LO, k0, below);
-                }
+                put_A(k0, delta);                            // A of the data gradient and GA of the reductions
+                if (h >= 2) st_row8(smem + S_GB, p, k0, below);
             };
             // directions first (pairs: second-order channel, then its first-order partner), the value channel last
             for (int gg = 1; gg <= NF + 1; ++gg) {
@@ -775,47 +693,25 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
             if (lane == 0) slot[3 + i] = v;
         }
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    if (kh == 0) {
-        // M = 64 accumulators: row j sits in lane (j % 16) + 32 (j / 16); the second K half of the same sum sits 16
-        // lanes higher and is added here
-        const int half = lane >> 4, j = 16 * warp + (lane & 15);
-        auto both8 = [&](int col, float (&v)[8]) {
-            tmem_ld8(tm_lane + col, v);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] += __shfl_xor_sync(0xffffffffu, v[i], 16);
-        };
+    {
+        const float* wacc = reinterpret_cast<const float*>(smem + S_WACC);
+        const float* smallh = reinterpret_cast<const float*>(smem + S_SMALLH);
         for (int li = 0; li + 2 < Ln; ++li) {               // hidden->hidden layer li+1
             const DevLayer& L = P.layer[li + 1];
-            for (int m0 = 0; m0 < rup(L.n_in, 8); m0 += 8) {
-                float v[8];
-                both8(TM_WACC + 64 * li + m0, v);
-                if (half == 0 && j < L.n_out) {
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) if (m0 + i < L.n_in) mine[L.w_off + j * L.n_in + m0 + i] = v[i];
-                }
-            }
-            float v[8];
-            both8(TM_SMALLH + 8 * li, v);                    // level li+2: bias gradient of layer li+1
-            if (half == 0 && j < L.n_out) mine[L.b_off + j] = v[0];
+            for (int i = tid; i < L.n_out * L.n_in; i += NT)
+                mine[L.w_off + i] = wacc[li * KW * KW + (i / L.n_in) * KW + i % L.n_in];
+            for (int j = tid; j < L.n_out; j += NT) mine[L.b_off + j] = smallh[li * KW * 8 + j * 8];   // bias gradient
         }
-        {
-            const DevLayer& L0 = P.layer[0];
-            float v[8], w[8];
-            both8(TM_SMALL1, v);
-            both8(TM_SMALL1 + 8, w);
-            if (half == 0 && j < L0.n_out) {
-                mine[L0.b_off + j] = v[0];
-#pragma unroll
-                for (int i = 0; i < PINN_MAX_DIMS; ++i)
-                    if (i < L0.n_in) mine[L0.w_off + j * L0.n_in + i] = (i < 7) ? v[1 + i] : w[0];
-            }
-            const DevLayer& LO = P.layer[H];
-            both8(TM_OUT, v);
-            if (half == 0 && j < LO.n_in) mine[LO.w_off + j] = v[0];
+        const float* small1 = reinterpret_cast<const float*>(smem + S_SMALL1);   // [j][0] bias, [j][1 + i] weights
+        const DevLayer& L0 = P.layer[0];
+        for (int j = tid; j < L0.n_out; j += NT) {
+            mine[L0.b_off + j] = small1[j * 16];
+            for (int i = 0; i < L0.n_in; ++i) mine[L0.w_off + j * L0.n_in + i] = small1[j * 16 + 1 + i];
         }
+        const float* outw = reinterpret_cast<const float*>(smem + S_OUT);
+        const DevLayer& LO = P.layer[H];
+        for (int j = tid; j < LO.n_in; j += NT) mine[LO.w_off + j] = outw[j * 8];
     }
     if (tid == 0) {
         float sc[3 + PINN_MAX_VARS];
@@ -830,9 +726,7 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
         mine[P.layer[H].b_off] = sc[2];
         for (int i = 0; i < P.n_vars; ++i) mine[P.var_off[i]] = sc[3 + i];
     }
-    tc_fence_before();
     __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" :: "r"(mc.tmem) : "memory");
     finish_grid(a, n_out_floats);
 }
 

@@ -1,4 +1,4 @@
-// wide_step_kernel (tcgen05 / TMEM tile kernel for wide networks) instantiations for NF = 4 first-order directions
+// wide_step_kernel (tensor-core tile kernel for wide networks) instantiations for NF = 4 first-order directions
 #include "pinn_wide_kernel.cuh"
 
 pinn::StepKernelFn pinn_wide_variant_nf4(int ns, int threads) {

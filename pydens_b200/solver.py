@@ -1,4 +1,4 @@
-""" `Solver` — the pydens user API (reference pydens/model_torch.py:191-487) on the B200 engine.
+""" `Solver` — the pydens user API (reference pydens/model_torch.py:191-487) on the H100 engine.
 
 Same constructor, `fit`, `predict`, `reshape_and_concat`, attributes (`model`, `losses`, `optimizer`,
 `ctx`, `equation`, `constraints`).  What changes is the body of the training loop: where the

@@ -40,7 +40,7 @@ def test_two_gpu_fit_matches_single_gpu(tmp_path):
 
 @pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason='needs 2 GPUs')
 def test_two_gpu_tile_kernel_fit_matches_single_gpu(tmp_path):
-    """ cfg5's network (tcgen05 tile kernel, 51 KB gradient vector through the in-kernel NVLink all-reduce): the
+    """ cfg5's network (tensor-core tile kernel, 51 KB gradient vector through the in-kernel NVLink all-reduce): the
     2-GPU fit on uneven shards of the same global batch follows the single-GPU fit. """
     one = _run(1, str(tmp_path / 'w1.json'), problem='wave3d')
     two = _run(2, str(tmp_path / 'w2.json'), problem='wave3d')

@@ -1,4 +1,4 @@
-""" The tcgen05 / TMEM tile kernel for wide networks (pydens_b200/csrc/pinn_wide_kernel.cuh) against the reference's
+""" The tensor-core tile kernel for wide networks (pydens_b200/csrc/pinn_wide_kernel.cuh) against the reference's
 goldens, the oracle port, and the thread-per-point kernel.  `PINN_FORCE_KERNEL=wide` puts the tile kernel on every
 problem it covers (plain dense chains, tanh / sigmoid / identity activations, hidden widths <= 64), so that its
 3xTF32 arithmetic is held to the same fp32 tolerances as the CUDA-core kernel: loss rel <= 1e-5, residual rel-L2

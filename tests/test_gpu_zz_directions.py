@@ -65,10 +65,12 @@ def test_fit_trajectory_matches_reference_fit(name, adam, monkeypatch):
 def test_ragged_batches_against_oracle(n):
     g = load_golden('hess3d')
     solver = make_solver('hess3d', g['params'])
-    prob = oracle_problem('hess3d', torch.float32, g['params'])
+    # the fp64 oracle: the fp32 one carries its own rounding, which depends on the host CPU's kernels (3.6e-5 residual
+    # error at one of these points on some hosts, while the device result stays within 1.3e-7 of fp64)
+    prob = oracle_problem('hess3d', torch.float64, g['params'])
     pts = P.make_points('hess3d', n, seed=77)
     loss, grads, residual = solver.loss_and_grads(pts)
-    l, r, gr = prob.loss_and_grads(pts)
+    l, r, gr = prob.loss_and_grads(torch.as_tensor(pts, dtype=torch.float64))
     assert abs(loss - l) <= 1e-5 * abs(l)
     assert rel_l2(residual.cpu().numpy(), r) <= 1e-5
     assert rel_l2(grads.cpu().numpy(), gr.numpy()) <= 1e-4

@@ -1,6 +1,6 @@
 """ Criteria other than MSELoss on the GPU (reference model_torch.py:365, :448 `criterion(residual, zeros)`): L1Loss,
 HuberLoss and SmoothL1Loss train on the same kernels through the residual transform of tracer.apply_criterion —
-through the bare C ABI against torch's own criteria on the fp64 oracle (thread kernel, tcgen05 tile kernel, whole-jet
+through the bare C ABI against torch's own criteria on the fp64 oracle (thread kernel, tensor-core tile kernel, whole-jet
 kernel), and through Solver.fit against the oracle port of the reference loop on identical batches.  (Sorted last: this
 joined after the round's GPU time was spent; its CPU twin is test_emul.py::test_other_criteria_ride_on_the_mse_kernels.) """
 import numpy as np

@@ -37,7 +37,7 @@ def main():
         solver = Solver(pde, ndims=2, boundary_condition=1, layout='fa fa fa f', activation='Tanh',
                         units=[10, 12, 15, 1], device=torch.device('cuda', local), backend='fused', seed=7)
         solver.fit(niters=30, batch_size=100001, lr=0.005)          # odd size: uneven shards
-    else:                                  # a registry problem, e.g. wave3d: the tcgen05 tile kernel under data parallelism
+    else:                                  # a registry problem, e.g. wave3d: the tensor-core tile kernel under data parallelism
         import problems as P
         cfg = P.PROBLEMS[problem]
         solver = Solver(P.bind(problem, D, lambda n, init: V(n, data=torch.Tensor([init]))), ndims=cfg['ndims'],
