@@ -541,12 +541,26 @@ class Sym:
     def where(self, condition, other):
         return Sym(_where(condition, self, other))
 
+    # A traced value that depends on the points (u, its derivatives, the point columns) is one column, [N, 1].
+    # Selecting that column keeps the shape and is the identity: f[:, 0:1], f[:, [0]], f[..., 0:1], and splitting into
+    # one-column pieces.  f[:, 0] is [N] in torch (and then broadcasts to [N, N] against the [N, 1] columns), so it
+    # stays on autograd, as does any other index — and any index of a variable or constant, which is not [N, 1].
+    def __getitem__(self, key):
+        _column_of_index(_as_column(self), key)
+        return self
+
+    def split(self, size, dim=None):
+        return _split_columns(self, size, dim)
+
+    def chunk(self, chunks, dim=None):
+        return _chunk_columns(self, chunks, dim)
+
     # what a tensor would accept but a symbolic column cannot express: bail out of the fused path cleanly
     # (the reference runs such equations on autograd, model_torch.py:448) instead of raising a TypeError
     def _unsupported(self, *args, **kwargs):
         raise NotLowerable('indexing / integer arithmetic / len() on a traced tensor')
 
-    __getitem__ = __setitem__ = __mod__ = __rmod__ = __floordiv__ = __rfloordiv__ = _unsupported
+    __setitem__ = __mod__ = __rmod__ = __floordiv__ = __rfloordiv__ = _unsupported
     __len__ = __iter__ = __matmul__ = __rmatmul__ = _unsupported
     __int__ = __float__ = __index__ = _unsupported
 
@@ -558,6 +572,8 @@ class Sym:
     @classmethod
     def __torch_function__(cls, func, types, args=(), kwargs=None):
         name = getattr(func, '__name__', None)
+        if name in _COLUMN_FUNCS:
+            return _COLUMN_FUNCS[name](*args, **(kwargs or {}))
         if name in ('clamp', 'clip', 'clamp_min', 'clamp_max') and args and set(kwargs or ()) <= {'min', 'max'}:
             rest = list(args[1:])
             if name == 'clamp_max':
@@ -633,8 +649,115 @@ class Sym:
         raise NotLowerable('numpy.%s is not supported by the fused path' % ufunc.__name__)
 
 
+def _as_column(s):
+    """ `s` when it stands for an [N, 1] column of the batch: an expression of u or of the point columns.  A V(...)
+    variable is a one-element tensor and a constant a number in the reference; indexing, splitting or concatenating
+    those fails there (or means something else), so it is not lowered here either. """
+    if not leaves(s.expr, ('u', 'coord')):
+        raise NotLowerable('indexing / split / concatenation of a traced value that is not a column of the batch')
+    return s
+
+
+def _column_of_index(s, key):
+    """ Column selected by `key` when it keeps the [N, 1] shape (f[:, j:j+1], f[:, [j]], f[..., j:j+1]); a traced column
+    has one column, so only j = 0 exists. """
+    if not isinstance(key, tuple) or len(key) != 2 or not (key[0] is Ellipsis or key[0] == slice(None)):
+        raise NotLowerable('indexing a traced tensor other than f[:, j:j+1] / f[:, [j]]')
+    sel = key[1]
+    if isinstance(sel, slice) and sel.step in (None, 1) and isinstance(sel.start, int) and isinstance(sel.stop, int) \
+            and sel.start >= 0 and sel.stop == sel.start + 1:
+        j = sel.start
+    elif isinstance(sel, list) and len(sel) == 1 and isinstance(sel[0], int):
+        j = sel[0]
+    else:
+        raise NotLowerable('indexing a traced tensor other than f[:, j:j+1] / f[:, [j]] (f[:, j] is one-dimensional)')
+    if j not in (0, -1):
+        raise NotLowerable('column %d of a one-column traced tensor' % j)
+    return 0
+
+
+def _column_dim(dim):
+    if dim not in (1, -1):
+        raise NotLowerable('split / concatenation of traced tensors along dimension %r (only the column one)' % (dim,))
+
+
+def _split_columns(s, size, dim=None):
+    """ torch.split(f, 1, dim=1) / f.split(1, 1) of a one-column value: that column. """
+    _as_column(s)
+    _column_dim(dim)
+    if not (size >= 1 if isinstance(size, int) else isinstance(size, (list, tuple)) and list(size) == [1]):
+        raise NotLowerable('torch.split of a traced tensor with sizes %r' % (size,))
+    return (s,)
+
+
+def _chunk_columns(s, chunks, dim=None):
+    _as_column(s)
+    _column_dim(dim)
+    if not (isinstance(chunks, int) and chunks >= 1):
+        raise NotLowerable('torch.chunk of a traced tensor into %r chunks' % (chunks,))
+    return (s,)
+
+
+def _concat_columns(tensors, dim=None, axis=None, hstack=False):
+    """ torch.cat([r_1, …, r_m], dim=1) and its spellings: a residual of m columns (VecSym). """
+    if not hstack:
+        _column_dim(dim if axis is None else axis)
+    cols = []
+    for t in tensors:
+        if isinstance(t, VecSym):
+            cols += t.exprs
+        elif isinstance(t, Sym):
+            cols.append(_as_column(t).expr)
+        else:
+            raise NotLowerable('concatenation of a traced value with a %s' % type(t).__name__)
+    if not cols:
+        raise NotLowerable('empty concatenation')
+    return Sym(cols[0]) if len(cols) == 1 else VecSym(cols)
+
+
+_COLUMN_FUNCS = {
+    'cat': lambda tensors, dim=0: _concat_columns(tensors, dim),
+    'concat': lambda tensors, dim=0: _concat_columns(tensors, dim),
+    'concatenate': lambda tensors, axis=0: _concat_columns(tensors, axis),
+    'hstack': lambda tensors: _concat_columns(tensors, hstack=True),
+    'column_stack': lambda tensors: _concat_columns(tensors, hstack=True),
+    'split': lambda s, size, dim=0: _split_columns(s, size, dim),
+    'chunk': lambda s, chunks, dim=0: _chunk_columns(s, chunks, dim),
+}
+
+
+class VecSym:
+    """ Symbolic stand-in for an `[N, m]` residual, m > 1: the columns r_1 … r_m, as `torch.cat` of one-column values
+    returns it.  It can only be returned by the equation (or concatenated further); the loss of the reference,
+    `criterion(residual, zeros[N, 1])`, broadcasts over the m columns (model_torch.py:448). """
+
+    def __init__(self, exprs):
+        self.exprs = list(exprs)
+
+    @classmethod
+    def __torch_function__(cls, func, types, args=(), kwargs=None):
+        name = getattr(func, '__name__', None)
+        if name in ('cat', 'concat', 'concatenate', 'hstack', 'column_stack'):
+            return _COLUMN_FUNCS[name](*args, **(kwargs or {}))
+        raise NotLowerable('torch.%s of a residual with several columns' % name)
+
+    def __getattr__(self, name):
+        if name.startswith('__'):
+            raise AttributeError(name)
+        raise NotLowerable('%r of a residual with several columns' % name)
+
+    def _unsupported(self, *args, **kwargs):
+        raise NotLowerable('arithmetic / indexing on a residual with several columns')
+
+    __add__ = __radd__ = __sub__ = __rsub__ = __mul__ = __rmul__ = __truediv__ = __rtruediv__ = _unsupported
+    __pow__ = __rpow__ = __neg__ = __abs__ = __getitem__ = __len__ = __iter__ = __bool__ = _unsupported
+    __array_ufunc__ = None
+
+
 def sym_D(y, x):
     """ Symbolic counterpart of the D token. """
+    if isinstance(y, VecSym):
+        raise NotLowerable('D() of a residual with several columns')
     if not isinstance(x, Sym) or x.expr.kind != 'coord':
         raise NotLowerable('D(y, x): x must be one of the equation arguments')
     return Sym(diff_coord(_as_expr(y), x.expr.value))
@@ -835,6 +958,13 @@ def apply_criterion(res, criterion):
     residuals — where a fit ends up — do not lose digits against delta. """
     if criterion is None or criterion[0] == 'mse':
         return res
+    return unary('sqrt', add(criterion_rho(res, criterion), const(CRITERION_EPS)))
+
+
+def criterion_rho(res, criterion):
+    """ The criterion's pointwise function rho(r): r^2 for MSELoss, |r| for L1Loss, Huber's / SmoothL1's piecewise form. """
+    if criterion is None or criterion[0] == 'mse':
+        return powi(res, 2)
     kind = criterion[0]
     a = unary('abs', res)
     if kind == 'l1' or (kind == 'smooth_l1' and float(criterion[1]) == 0.0):
@@ -850,7 +980,7 @@ def apply_criterion(res, criterion):
             rho = mul(const(1.0 / delta), rho)
     else:
         raise NotLowerable('criterion %r' % (kind,))
-    return unary('sqrt', add(rho, const(CRITERION_EPS)))
+    return rho
 
 
 def criterion_outputs(res, partials, criterion):
@@ -865,25 +995,70 @@ def criterion_outputs(res, partials, criterion):
     return [substitute(g, {z: res})] + [mul(gp, p) for p in partials]
 
 
+def residual_outputs(rs, wrt, criterion):
+    """ Outputs of the residual program of an equation with residual columns `rs` (m of them): the residual the kernels
+    train on, then its partial w.r.t. every leaf of `wrt` (jet channels, then variables).
+
+    One column: `criterion_outputs`, the program of a scalar equation.  Several: the reference's loss
+    `criterion(residual[N, m], zeros[N, 1])` broadcasts, so it is the mean (reduction='sum': the sum) of rho(r_j) over
+    all N m entries.  The kernels train on ONE residual per point, so the columns are folded into
+        r~ = sqrt(s sum_j rho(r_j) + eps),   s = 1 / m (mean) or 1 (sum),
+    whose per-point weight 1 / N (or 1) gives exactly that loss plus eps, and whose adjoint seed
+    2 r~ dr~ = s sum_j rho'(r_j) dr_j is exact (the square root cancels, as in apply_criterion).  The derivative of r~
+    w.r.t. every r_j is taken once, on placeholder leaves, and shared by all partials. """
+    if len(rs) == 1:
+        return criterion_outputs(rs[0], [diff_leaf(rs[0], l) for l in wrt], criterion)
+    zs = [var('__residual_%d__' % j) for j in range(len(rs))]
+    total = ZERO
+    for z in zs:
+        total = add(total, criterion_rho(z, criterion))
+    scale = 1.0 if (criterion is not None and criterion[-1] == 'sum') else 1.0 / len(rs)
+    g = unary('sqrt', add(mul(const(scale), total), const(CRITERION_EPS)))
+    to_res = dict(zip(zs, rs))
+    gps = [substitute(diff_leaf(g, z), to_res) for z in zs]
+    outs = [substitute(g, to_res)]
+    for leaf in wrt:
+        acc = ZERO
+        for gp, r in zip(gps, rs):
+            p = diff_leaf(r, leaf)
+            if not is_const(p, 0.0):
+                acc = add(acc, mul(gp, p))
+        outs.append(acc)
+    return outs
+
+
+def _residual_columns(out):
+    """ The equation's return value as a list of per-point expressions (one per residual column). """
+    if isinstance(out, VecSym):
+        return list(out.exprs)
+    return [out.expr if isinstance(out, Sym) else _as_expr(out)]
+
+
+def _leaves_of(exprs, kinds):
+    seen, found = set(), []
+    for e in exprs:
+        leaves(e, kinds, seen, found)
+    return found
+
+
 def trace(equation, total, var_factory, initial_condition=None, ndims_spatial=0, run=None, criterion=None):
     """ Trace `equation(u, *xs)` (and `initial_condition(*x_spatial)` if callable).
 
     `var_factory(name)` is installed by the caller so that V(name, ...) returns `Sym(var(name))`
     during the trace.  `run` wraps the call (the Solver passes its contextvars ctx.run).
     `criterion`: see apply_criterion (default: the residual itself, MSE).
+    The equation may return one column or several (`torch.cat([...], dim=1)`): see residual_outputs.
     """
     run = run or (lambda f, *a: f(*a))
     xs = [Sym(coord(k)) for k in range(total)]
-    out = run(equation, Sym(uleaf()), *xs)
-    if not isinstance(out, Sym):
-        out = Sym(_as_expr(out))
-    res = out.expr
+    rs = _residual_columns(run(equation, Sym(uleaf()), *xs))
+    res = rs[0]
     T = TracedEquation()
     T.residual = res
 
-    u_leaves = leaves(res, ('u',))
+    u_leaves = _leaves_of(rs, ('u',))
     if any(len(l.value) > 2 for l in u_leaves):
-        return _trace_high_order(T, res, u_leaves, xs, total, initial_condition, ndims_spatial, run, criterion)
+        return _trace_high_order(T, rs, u_leaves, xs, total, initial_condition, ndims_spatial, run, criterion)
     first, second, mixed = set(), set(), set()
     for l in u_leaves:
         mi = l.value
@@ -922,8 +1097,9 @@ def trace(equation, total, var_factory, initial_condition=None, ndims_spatial=0,
         d = len(axes2) + n
         mapping[uleaf((i, j))] = mul(const(0.5), sub(sub(chleaf(1 + nf + d), mapping[uleaf((i, i))]),
                                                      mapping[uleaf((j, j))]))
-    res = substitute(res, mapping)
-    T.residual = apply_criterion(res, criterion)
+    memo = {}
+    rs = [substitute(r, mapping, memo) for r in rs]
+    res = rs[0]
     chan = {}
     by_channel = {c: chleaf(c) for c in range(C)}
 
@@ -938,13 +1114,13 @@ def trace(equation, total, var_factory, initial_condition=None, ndims_spatial=0,
         if leaves(ic, ('u',)):
             raise NotLowerable('initial_condition must not depend on the solution')
     ic_vars = {l.value for l in leaves(ic, ('var',))} if ic is not None else set()
-    T.var_names = sorted({l.value for l in leaves(res, ('var',))} | ic_vars)
+    T.var_names = sorted({l.value for l in _leaves_of(rs, ('var',))} | ic_vars)
     if len(T.var_names) > 4:
         raise NotLowerable('more than 4 trainable variables')
     var_index = {n: i for i, n in enumerate(T.var_names)}
 
-    outputs = criterion_outputs(res, [diff_leaf(res, by_channel[c]) for c in range(C)] + [diff_leaf(res, var(n)) for n in T.var_names],
-                                criterion)
+    outputs = residual_outputs(rs, [by_channel[c] for c in range(C)] + [var(n) for n in T.var_names], criterion)
+    T.residual = apply_criterion(res, criterion) if len(rs) == 1 else outputs[0]
     T.eq_prog = lower(outputs, chan, var_index, C)
     T.n_slots = T.eq_prog.n_slots
 
@@ -969,7 +1145,7 @@ def trace(equation, total, var_factory, initial_condition=None, ndims_spatial=0,
     return T
 
 
-def _trace_high_order(T, res, u_leaves, xs, total, initial_condition, ndims_spatial, run, criterion=None):
+def _trace_high_order(T, rs, u_leaves, xs, total, initial_condition, ndims_spatial, run, criterion=None):
     """ Equations with derivatives of order 3 / 4 (D nested three / four times: u_xxx, u_xxxx): every direction carries
     its whole Taylor jet up to the highest order met (pinn_device_hi.cuh).  Directions are the differentiated
     arguments and, for every pair (i, j) with a mixed derivative, the two diagonals p = e_i + e_j and m = e_i - e_j,
@@ -1019,10 +1195,11 @@ def _trace_high_order(T, res, u_leaves, xs, total, initial_condition, ndims_spat
         if order >= 4:
             mapping[uleaf((i, i, j, j))] = mul(const(1.0 / 12.0), sub(sub(add(ch(dp, 4), ch(dm, 4)), mul(const(2.0), ch(di, 4))),
                                                                     mul(const(2.0), ch(dj, 4))))
-    res = substitute(res, mapping)
-    if leaves(res, ('u',)):
+    memo = {}
+    rs = [substitute(r, mapping, memo) for r in rs]
+    res = rs[0]
+    if _leaves_of(rs, ('u',)):
         raise NotLowerable('a derivative of the equation has no jet channel')
-    T.residual = apply_criterion(res, criterion)
 
     ic = None
     if initial_condition is not None:
@@ -1034,14 +1211,14 @@ def _trace_high_order(T, res, u_leaves, xs, total, initial_condition, ndims_spat
         if leaves(ic, ('u',)):
             raise NotLowerable('initial_condition must not depend on the solution')
     ic_vars = {l.value for l in leaves(ic, ('var',))} if ic is not None else set()
-    T.var_names = sorted({l.value for l in leaves(res, ('var',))} | ic_vars)
+    T.var_names = sorted({l.value for l in _leaves_of(rs, ('var',))} | ic_vars)
     if len(T.var_names) > 4:
         raise NotLowerable('more than 4 trainable variables')
     if 1 + C + len(T.var_names) > 2 + 2 * MAX_DIRS + 4 or (ic_vars and C * (1 + len(T.var_names)) > (1 + 2 * MAX_DIRS) * 5):
         raise NotLowerable('%d jet channels and %d variables exceed the outputs of a residual program' % (C, len(T.var_names)))
     var_index = {n: i for i, n in enumerate(T.var_names)}
-    outputs = criterion_outputs(res, [diff_leaf(res, chleaf(c)) for c in range(C)] + [diff_leaf(res, var(n)) for n in T.var_names],
-                                criterion)
+    outputs = residual_outputs(rs, [chleaf(c) for c in range(C)] + [var(n) for n in T.var_names], criterion)
+    T.residual = apply_criterion(res, criterion) if len(rs) == 1 else outputs[0]
     T.eq_prog = lower(outputs, {}, var_index, C)
     T.n_slots = T.eq_prog.n_slots
     if ic is not None:
