@@ -130,10 +130,16 @@ PINN_HD uint32_t philox_word(const Philox4& p, int i) {
     return i == 0 ? p.x : (i == 1 ? p.y : (i == 2 ? p.z : p.w));
 }
 
-// Coordinate k of the point with global index `gidx` at step `step`.
+// Block `block` of the point with global index `gidx` at step `step`.
 // Counter = (gidx lo, gidx hi, step lo, (step hi & 0xffff) << 16 | block); key = seed.
-// block 0/1 serve uniform columns 0-3 / 4-7 (one word each); block 2+k serves normal column k;
-// block 10+g, word 0 picks the component of mixture group g.
+// block 0/1 serve uniform columns 0-3 / 4-7 (one word each); block 2+k serves normal column k (attempt t of a
+// truncated normal: block 2+k | t << 8); block 10+g, word 0 picks the component of mixture group g.
+PINN_HD Philox4 philox_block(uint64_t gidx, uint64_t step, uint64_t seed, uint32_t block) {
+    return philox4x32_10((uint32_t)gidx, (uint32_t)(gidx >> 32), (uint32_t)step,
+                         (uint32_t)(((step >> 32) & 0xffffu) << 16) | block, (uint32_t)seed, (uint32_t)(seed >> 32));
+}
+
+// Coordinate k of the point with global index `gidx` at step `step` (blk0 / blk1: its blocks 0 and 1).
 PINN_HD float sample_simple(int kind, float a, float b, int k, uint64_t gidx, uint64_t step, uint64_t seed,
                             const Philox4& blk0, const Philox4& blk1) {
     if (kind == PINN_COL_CONST) return a;

@@ -51,13 +51,9 @@ __global__ void __launch_bounds__(256, 1) hi_step_kernel(const __grid_constant__
             for (int k = 0; k < P.total; ++k) st[k * RS] = __ldg(src + k);
         } else {
             const uint64_t gidx = a.point_offset + (uint64_t)pe;
-            const uint32_t c3 = (uint32_t)(((step >> 32) & 0xffffu) << 16);
-            Philox4 b0 = philox4x32_10((uint32_t)gidx, (uint32_t)(gidx >> 32), (uint32_t)step, c3,
-                                       (uint32_t)a.seed, (uint32_t)(a.seed >> 32));
+            Philox4 b0 = philox_block(gidx, step, a.seed, 0u);
             Philox4 b1 = b0;
-            if (P.total > 4)
-                b1 = philox4x32_10((uint32_t)gidx, (uint32_t)(gidx >> 32), (uint32_t)step, c3 | 1u,
-                                   (uint32_t)a.seed, (uint32_t)(a.seed >> 32));
+            if (P.total > 4) b1 = philox_block(gidx, step, a.seed, 1u);
             for (int k = 0; k < P.total; ++k) st[k * RS] = sample_column(P.cols[k], k, gidx, step, a.seed, b0, b1);
         }
         float r = point_step<NF, K>(P, sw, a.params, st, RS, valid, a.inv_n, sink, part);
@@ -90,9 +86,3 @@ __global__ void __launch_bounds__(256, 1) hi_step_kernel(const __grid_constant__
 
 }  // namespace hi
 }  // namespace pinn
-
-// one lookup function per direction count, each defined in its own translation unit (pinn_hi_nf*.cu)
-pinn::StepKernelFn pinn_hi_variant_nf1(int order);
-pinn::StepKernelFn pinn_hi_variant_nf2(int order);
-pinn::StepKernelFn pinn_hi_variant_nf3(int order);
-pinn::StepKernelFn pinn_hi_variant_nf4(int order);

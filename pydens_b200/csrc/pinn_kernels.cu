@@ -17,33 +17,28 @@
 #include <stdarg.h>
 #include <string.h>
 #include <stdlib.h>
+#include <memory>
 #include <new>
 
 #include "pinn_step_kernel.cuh"
 #include "pinn_wide_kernel.cuh"
 #include "pinn_small_kernel.cuh"
-#include "pinn_hi_kernel.cuh"
 #include "pinn_host_plan.h"
 
-// small_step_kernel instantiations live in pinn_small_nf*.cu
-pinn::MultiKernelFn pinn_small_variant_nf0(int ns);
-pinn::MultiKernelFn pinn_small_variant_nf1(int ns);
-pinn::MultiKernelFn pinn_small_variant_nf2(int ns);
-pinn::MultiKernelFn pinn_small_variant_nf3(int ns);
-pinn::MultiKernelFn pinn_small_variant_nf4(int ns);
-
-// wide_step_kernel instantiations live in pinn_wide_nf*.cu
-pinn::StepKernelFn pinn_wide_variant_nf0(int ns, int threads);
-pinn::StepKernelFn pinn_wide_variant_nf1(int ns, int threads);
-pinn::StepKernelFn pinn_wide_variant_nf2(int ns, int threads);
-pinn::StepKernelFn pinn_wide_variant_nf3(int ns, int threads);
-pinn::StepKernelFn pinn_wide_variant_nf4(int ns, int threads);
-
-// step_kernel instantiations for five / six derivative directions live in pinn_variants_hi_nf*.cu
-const pinn::Variant* pinn_variants_hi_nf5(int ns);
-const pinn::Variant* pinn_variants_hi_nf6(int ns);
-
 namespace pinn {
+
+// The kernel table, filled by the build units of pinn_instances.cu during static initialisation.  A function-local
+// static is initialised on first use, so the order in which the units initialise does not matter.
+KernelSet& kernel_slot(int nf, int ns, int order) {
+    static KernelSet table[3][PINN_MAX_DIRS + 1][PINN_MAX_DIRS + 1];      // [order - 2][nf][ns]
+    return table[order - 2][nf][ns];
+}
+
+const KernelSet* kernels(int nf, int ns, int order) {
+    if (order < 2 || order > 4 || nf < 0 || nf > PINN_MAX_DIRS || ns < 0 || ns > nf) return nullptr;
+    const KernelSet& k = kernel_slot(nf, ns, order);
+    return k.step[1][1] ? &k : nullptr;
+}
 
 // ---------------------------------------------------------------------------------------------------
 // Forward-only kernel (predict): u for explicit points.
@@ -103,7 +98,7 @@ __global__ void record_loss_kernel(const float* out, int loss_idx, float* ring, 
 }  // namespace pinn
 
 // ===================================================================================================
-// Host side: plan construction, variant dispatch, C ABI.
+// Host side: plan construction, kernel selection, C ABI.
 // ===================================================================================================
 using namespace pinn;
 
@@ -121,40 +116,8 @@ static int fail(int code, const char* fmt, ...) {
         if (e_ != cudaSuccess) return fail(PINN_E_CUDA, "%s: %s", #expr, cudaGetErrorString(e_)); \
     } while (0)
 
-// The function table of one (nf, ns): its two halves live in sibling translation units.
-static bool find_variant(int nf, int ns, Variant& out) {
-    if (ns < 0 || ns > nf) return false;
-    const Variant *a = nullptr, *b = nullptr;
-    switch (nf) {
-        case 0: a = pinn_variants_nf0(ns); b = pinn_variants_gen_nf0(ns); break;
-        case 1: a = pinn_variants_nf1(ns); b = pinn_variants_gen_nf1(ns); break;
-        case 2: a = pinn_variants_nf2(ns); b = pinn_variants_gen_nf2(ns); break;
-        case 3: a = pinn_variants_nf3(ns); b = pinn_variants_gen_nf3(ns); break;
-        case 4: a = pinn_variants_nf4(ns); b = pinn_variants_gen_nf4(ns); break;
-        // five / six directions: one kernel each (NS = NF, general form, per-point state in global memory)
-        case 5: a = b = pinn_variants_hi_nf5(ns); break;
-        case 6: a = b = pinn_variants_hi_nf6(ns); break;
-        default: return false;
-    }
-    if (!a || !b) return false;
-    out = *a;
-    out.smem_gen_fn = b->smem_gen_fn; out.gmem_gen_fn = b->gmem_gen_fn; out.multi_fn = b->multi_fn;
-    return true;
-}
-
 // The tensor-core tile kernel (pinn_wide_kernel.cuh) covers plain dense chains with polynomial-family activations
 // and hidden widths <= 64; it pays off once the layers are wide enough to be real GEMMs.
-static pinn::StepKernelFn find_wide_variant(int nf, int ns, int threads) {
-    if (ns < 0 || ns > nf) return nullptr;
-    switch (nf) {
-        case 0: return pinn_wide_variant_nf0(ns, threads);
-        case 1: return pinn_wide_variant_nf1(ns, threads);
-        case 2: return pinn_wide_variant_nf2(ns, threads);
-        case 3: return pinn_wide_variant_nf3(ns, threads);
-        case 4: return pinn_wide_variant_nf4(ns, threads);
-    }
-    return nullptr;
-}
 static bool wide_eligible(const pinn::DevPlan& h, int* max_width) {
     if (h.n_layers < 2 || h.n_layers > pinn::wide::MAX_LAYERS) return false;
     int mw = 0;
@@ -179,8 +142,7 @@ struct PinnPlan {
     MultiKernelFn fn_small;                  // tiny-batch (<= 128 points) variant, or nullptr
     int small_smem;
     int wide_ctas;                           // CTAs the tile kernel runs on (<= sm_count)
-    Variant var_store;
-    const Variant* var;
+    const KernelSet* ks;                     // the kernels of this plan's jet set
     StepKernelFn fn_smem, fn_gmem;           // the pair matching this plan (plain or general)
     int sm_count;
     int smem_optin;
@@ -206,195 +168,189 @@ static cudaError_t allow_max_smem(const void* fn, int smem_optin) {
     return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin - (int)fa.sharedSizeBytes);
 }
 
-extern "C" int pinn_plan_create(const PinnSpec* s, int device, PinnPlan** out) {
-    if (!s || !out) return fail(PINN_E_INVALID, "null argument");
-    const Variant* var = nullptr;
-    PinnPlan* p = new (std::nothrow) PinnPlan();
-    if (!p) return fail(PINN_E_INVALID, "out of memory");
-    {
-        char msg[256];
-        int rc = build_dev_plan(s, p->h, p->fwd_rows, p->fwd_row_scr, msg, sizeof(msg));
-        if (rc) { delete p; return fail(rc, "%s", msg); }
-    }
-    const int order = spec_order(s);
-    if (order >= 3) {
-        // derivatives of order 3 / 4: whole jets per direction (pinn_hi_kernel.cuh), one kernel per (nf, order)
-        StepKernelFn f = s->nf == 1 ? pinn_hi_variant_nf1(order) : s->nf == 2 ? pinn_hi_variant_nf2(order)
-                       : s->nf == 3 ? pinn_hi_variant_nf3(order) : s->nf == 4 ? pinn_hi_variant_nf4(order) : nullptr;
-        if (!f) { delete p; return fail(PINN_E_UNSUPPORTED, "no kernel for derivative order %d with %d directions", order, s->nf); }
-        const Variant v = {s->nf, 0, nullptr, nullptr, nullptr, f, nullptr, 256};
-        p->var_store = v;
-    } else if (!find_variant(s->nf, s->ns, p->var_store)) {
-        delete p;
-        return fail(PINN_E_UNSUPPORTED, "no kernel variant for nf=%d ns=%d%s", s->nf, s->ns,
-                    s->nf > 4 ? " (more than 4 derivative directions: every direction must carry its second derivative, ns = nf)" : "");
-    }
-    var = &p->var_store;
-    p->fn_smem = p->h.general ? var->smem_gen_fn : var->smem_fn;
-    p->fn_gmem = p->h.general ? var->gmem_gen_fn : var->gmem_fn;
-    // variants that exist in the general form only (nf > 4) serve plain plans with it; without a shared-memory
-    // resident instantiation the per-point state goes to the global area
-    if (!p->fn_gmem) p->fn_gmem = var->gmem_gen_fn;
+// Warps per CTA a kernel compiled for `maxt` threads can run at its register count (one CTA per SM).
+static int max_warps(const cudaFuncAttributes& fa, int maxt) {
+    const int by_regs = 65536 / (fa.numRegs * 32);
+    return by_regs < maxt / 32 ? by_regs : maxt / 32;
+}
+
+// Floats of the per-point storage area for `nw` warps of `rows` rows; the area holds at least the flat parameters.
+static int storage_floats(const DevPlan& h, int rows, int nw) {
+    return rows * RS * nw > h.n_params ? rows * RS * nw : h.n_params;
+}
+
+// Thread kernel: per-point state in shared memory at the largest warp count that fits (per-warp accumulators when
+// they fit too, else one shared accumulator with atomics), or in the global spill area.
+static int place_step_kernel(PinnPlan* p) {
+    const DevPlan& h = p->h;
+    const int n_out_floats = h.n_params + 4;
     const bool has_smem_form = p->fn_smem != nullptr;
-    if (!p->fn_gmem) { delete p; return fail(PINN_E_UNSUPPORTED, "no kernel variant for nf=%d ns=%d", s->nf, s->ns); }
-    p->spec = *s;
-    p->device = device;
-    p->var = var;
-    DevPlan& h = p->h;
-    cudaError_t e;
-
-    // ---- device queries and launch configuration ----
-    e = cudaSetDevice(device);
-    if (e != cudaSuccess) { delete p; return fail(PINN_E_CUDA, "cudaSetDevice(%d): %s", device, cudaGetErrorString(e)); }
-    cudaDeviceProp prop;
-    e = cudaGetDeviceProperties(&prop, device);
-    if (e != cudaSuccess) { delete p; return fail(PINN_E_CUDA, "cudaGetDeviceProperties: %s", cudaGetErrorString(e)); }
-    if (prop.major != 9 || prop.minor != 0) { delete p; return fail(PINN_E_UNSUPPORTED, "device sm_%d%d: this library is built for sm_90a only", prop.major, prop.minor); }
-    p->sm_count = prop.multiProcessorCount;
-    p->smem_optin = (int)prop.sharedMemPerBlockOptin;
-
-    const int n_out_floats = s->n_params + 4;
     cudaFuncAttributes fa;
-    e = cudaFuncGetAttributes(&fa, (const void*)(has_smem_form ? p->fn_smem : p->fn_gmem));
-    if (e != cudaSuccess) { delete p; return fail(PINN_E_CUDA, "cudaFuncGetAttributes: %s", cudaGetErrorString(e)); }
+    cudaError_t e = cudaFuncGetAttributes(&fa, (const void*)(has_smem_form ? p->fn_smem : p->fn_gmem));
+    if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncGetAttributes: %s", cudaGetErrorString(e));
     p->regs = fa.numRegs;
-    int max_warps_regs = (65536 / (fa.numRegs * 32));
-    int max_warps = var->maxt / 32;
-    if (max_warps_regs < max_warps) max_warps = max_warps_regs;
-    // shared-memory resident activations: largest warp count that fits (per-warp accumulators
-    // when they fit too, else one shared accumulator with atomics)
+    const int max_nw = max_warps(fa, p->ks->maxt);
     const int budget = p->smem_optin - (int)fa.sharedSizeBytes - 64;
     int best_nw = 0, best_nwacc = 0;
-    for (int nw = max_warps; nw >= 1 && !best_nw; --nw) {
+    for (int nw = max_nw; nw >= 1 && !best_nw; --nw) {
         for (int pass = 0; pass < 2 && !best_nw; ++pass) {
             int nwacc = pass == 0 ? nw : 1;
-            SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, nwacc,
-                                        h.rows_total * RS * nw > h.n_params ? h.rows_total * RS * nw : h.n_params);
+            SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, nwacc, storage_floats(h, h.rows_total, nw));
             if (SL.total_f * 4 <= budget) { best_nw = nw; best_nwacc = nwacc; }
         }
     }
     // PINN_FORCE_MODE=smem|gmem overrides the placement heuristic (experiments only)
     const char* force = getenv("PINN_FORCE_MODE");
-    bool use_smem = best_nw >= 4 || (best_nw >= 2 && max_warps <= 4);
+    bool use_smem = best_nw >= 4 || (best_nw >= 2 && max_nw <= 4);
     if (force && !strcmp(force, "smem") && best_nw >= 1) use_smem = true;
     if (force && !strcmp(force, "gmem")) use_smem = false;
     if (!has_smem_form) use_smem = false;
     if (use_smem) {
         p->gmem = false; p->threads = best_nw * 32; p->n_wacc = best_nwacc;
-        SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, best_nwacc,
-                                    h.rows_total * RS * best_nw > h.n_params ? h.rows_total * RS * best_nw : h.n_params);
+        SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, best_nwacc, storage_floats(h, h.rows_total, best_nw));
         p->smem_bytes = SL.total_f * 4;
     } else {
         // activations spill to a global workspace; accumulators: per warp if they fit, else shared
         e = cudaFuncGetAttributes(&fa, (const void*)p->fn_gmem);
-        if (e != cudaSuccess) { delete p; return fail(PINN_E_CUDA, "cudaFuncGetAttributes: %s", cudaGetErrorString(e)); }
+        if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncGetAttributes: %s", cudaGetErrorString(e));
         p->regs = fa.numRegs;
-        int nw = var->maxt / 32;
-        if (65536 / (fa.numRegs * 32) < nw) nw = 65536 / (fa.numRegs * 32);
+        int nw = max_warps(fa, p->ks->maxt);
         { const char* e2 = getenv("PINN_GMEM_WARPS"); if (e2 && atoi(e2) >= 1 && atoi(e2) <= nw) nw = atoi(e2); }   // experiments
         int nwacc = nw;
         SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, nwacc, h.n_params);
         if (SL.total_f * 4 > budget) { nwacc = 1; SL = smem_layout(h.weights_floats, n_out_floats, 1, h.n_params); }
-        if (SL.total_f * 4 > budget) { delete p; return fail(PINN_E_UNSUPPORTED, "network too large: %d B of weights do not fit shared memory", SL.total_f * 4); }
+        if (SL.total_f * 4 > budget) return fail(PINN_E_UNSUPPORTED, "network too large: %d B of weights do not fit shared memory", SL.total_f * 4);
         p->gmem = true; p->threads = nw * 32; p->n_wacc = nwacc; p->smem_bytes = SL.total_f * 4;
     }
     e = allow_max_smem((const void*)(p->gmem ? p->fn_gmem : p->fn_smem), p->smem_optin);
-    if (e != cudaSuccess) { delete p; return fail(PINN_E_CUDA, "cudaFuncSetAttribute(smem=%d): %s", p->smem_bytes, cudaGetErrorString(e)); }
+    if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(smem=%d): %s", p->smem_bytes, cudaGetErrorString(e));
+    return PINN_OK;
+}
 
-    // forward kernel config
-    {
-        int nw = 8;
-        SmemLayout SL = smem_layout(h.weights_floats, 0, 0, p->fwd_rows * RS * nw > h.n_params ? p->fwd_rows * RS * nw : h.n_params);
-        if (SL.total_f * 4 <= p->smem_optin - 64) { p->fwd_gmem = false; }
-        else { p->fwd_gmem = true; SL = smem_layout(h.weights_floats, 0, 0, h.n_params); }
-        p->fwd_threads = nw * 32; p->fwd_smem_bytes = SL.total_f * 4;
-        if (p->fwd_smem_bytes > p->smem_optin - 64) { delete p; return fail(PINN_E_UNSUPPORTED, "network too large for shared memory"); }
-        e = allow_max_smem((const void*)(p->fwd_gmem ? forward_kernel<true> : forward_kernel<false>), p->smem_optin);
-        if (e != cudaSuccess) { delete p; return fail(PINN_E_CUDA, "cudaFuncSetAttribute(fwd): %s", cudaGetErrorString(e)); }
-    }
+// Forward kernel: eight warps, per-point state in shared memory when it fits, else in the global spill area.
+static int place_forward_kernel(PinnPlan* p) {
+    const DevPlan& h = p->h;
+    const int nw = 8;
+    SmemLayout SL = smem_layout(h.weights_floats, 0, 0, storage_floats(h, p->fwd_rows, nw));
+    if (SL.total_f * 4 <= p->smem_optin - 64) { p->fwd_gmem = false; }
+    else { p->fwd_gmem = true; SL = smem_layout(h.weights_floats, 0, 0, h.n_params); }
+    p->fwd_threads = nw * 32; p->fwd_smem_bytes = SL.total_f * 4;
+    if (p->fwd_smem_bytes > p->smem_optin - 64) return fail(PINN_E_UNSUPPORTED, "network too large for shared memory");
+    const cudaError_t e = allow_max_smem((const void*)(p->fwd_gmem ? forward_kernel<true> : forward_kernel<false>), p->smem_optin);
+    if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(fwd): %s", cudaGetErrorString(e));
+    return PINN_OK;
+}
 
-    // ---- persistent multi-step kernel (small batches): per-point state + parameters + Adam moments in shared memory ----
-    {
-        p->fn_multi = nullptr; p->multi_threads = 0; p->multi_nwacc = 0; p->multi_smem = 0;
-        if (var->multi_fn) {
-            cudaFuncAttributes fm;
-            e = cudaFuncGetAttributes(&fm, (const void*)var->multi_fn);
-            if (e == cudaSuccess) {
-                int mw = var->maxt / 32;
-                if (65536 / (fm.numRegs * 32) < mw) mw = 65536 / (fm.numRegs * 32);
-                const int extra = 3 * align4(h.n_params) + align4(n_out_floats);
-                const int mbudget = p->smem_optin - (int)fm.sharedSizeBytes - 64;
-                for (int nw = mw; nw >= 1 && !p->fn_multi; --nw) {
-                    SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, nw,
-                                                h.rows_total * RS * nw > h.n_params ? h.rows_total * RS * nw : h.n_params);
-                    if ((SL.total_f + extra) * 4 <= mbudget) {
-                        p->fn_multi = var->multi_fn; p->multi_threads = nw * 32; p->multi_nwacc = nw;
-                        p->multi_smem = (SL.total_f + extra) * 4;
-                    }
-                }
-                if (p->fn_multi) {
-                    e = allow_max_smem((const void*)p->fn_multi, p->smem_optin);
-                    if (e != cudaSuccess) p->fn_multi = nullptr;
-                }
+// Persistent multi-step kernel (small batches): per-point state + parameters + Adam moments in shared memory.  Left
+// out when the jet set has none or the network does not fit.
+static void place_multi_kernel(PinnPlan* p) {
+    p->fn_multi = nullptr; p->multi_threads = 0; p->multi_nwacc = 0; p->multi_smem = 0;
+    const MultiKernelFn f = p->ks->multi;
+    if (!f) return;
+    cudaFuncAttributes fm;
+    if (cudaFuncGetAttributes(&fm, (const void*)f) == cudaSuccess) {
+        const DevPlan& h = p->h;
+        const int n_out_floats = h.n_params + 4;
+        const int extra = 3 * align4(h.n_params) + align4(n_out_floats);
+        const int mbudget = p->smem_optin - (int)fm.sharedSizeBytes - 64;
+        for (int nw = max_warps(fm, p->ks->maxt); nw >= 1 && !p->fn_multi; --nw) {
+            SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, nw, storage_floats(h, h.rows_total, nw));
+            if ((SL.total_f + extra) * 4 <= mbudget) {
+                p->fn_multi = f; p->multi_threads = nw * 32; p->multi_nwacc = nw;
+                p->multi_smem = (SL.total_f + extra) * 4;
             }
-            (void)cudaGetLastError();
         }
+        if (p->fn_multi && allow_max_smem((const void*)f, p->smem_optin) != cudaSuccess) p->fn_multi = nullptr;
     }
+    (void)cudaGetLastError();
+}
 
-    // ---- tiny batches: the (point, unit)-parallel loop kernel; plain dense chains whose jets fit shared memory ----
+// Tiny batches: the (point, unit)-parallel loop kernel, for plain dense chains whose jets fit shared memory.  Left out
+// when the jet set has none (more than four directions, orders 3 / 4).
+static void place_small_kernel(PinnPlan* p) {
+    p->fn_small = nullptr; p->small_smem = 0;
+    const MultiKernelFn f = p->ks->small;
+    if (!f) return;
+    const DevPlan& h = p->h;
+    for (int l = 0; l < h.n_layers; ++l) if (h.layer[l].skip_src >= 0 || h.layer[l].post_base >= 0) return;
+    const int bytes = small::make_layout(h).total * 4;
+    cudaFuncAttributes fs;
+    if (cudaFuncGetAttributes(&fs, (const void*)f) == cudaSuccess && bytes <= p->smem_optin - (int)fs.sharedSizeBytes - 64 &&
+        allow_max_smem((const void*)f, p->smem_optin) == cudaSuccess) {
+        p->fn_small = f; p->small_smem = bytes;
+    }
+    (void)cudaGetLastError();
+}
+
+// Wide networks: the tensor-core tile kernel takes the step (PINN_FORCE_KERNEL=thread|wide overrides).
+static int place_wide_kernel(PinnPlan* p, int order) {
+    p->wide = false; p->fn_wide = nullptr; p->wide_ctas = p->sm_count;
+    int mw = 0;
+    const char* fk = getenv("PINN_FORCE_KERNEL");
+    const bool eligible = order < 3 && wide_eligible(p->h, &mw);
+    // the tile kernel wins from 64-wide layers with many jet channels on (H100 80GB HBM3 at 700 W, cfg5: 21.1 ms
+    // vs 32.3 ms per step); for narrower networks the per (unit, channel) operand handling costs as much as the
+    // FMA row it replaces, and the CUDA-core kernel keeps them
+    bool want = eligible && mw >= 48 && (1 + p->spec.nf + p->spec.ns) >= 5;
+    if (fk && !strcmp(fk, "thread")) want = false;
+    if (fk && !strcmp(fk, "wide")) {
+        if (!eligible) return fail(PINN_E_UNSUPPORTED, "PINN_FORCE_KERNEL=wide: this network is outside what the tile kernel covers");
+        want = true;
+    }
+    int wide_threads = 512;                     // four threads per point; PINN_WIDE_THREADS=256: two (experiments)
+    { const char* wt = getenv("PINN_WIDE_THREADS"); if (wt && atoi(wt) == 256) wide_threads = 256; }
+    const StepKernelFn f = p->ks->wide[wide_threads == 256 ? 1 : 0];
+    if (!want || !f) return PINN_OK;
+    cudaError_t e = cudaFuncSetAttribute((const void*)f, cudaFuncAttributeMaxDynamicSharedMemorySize, wide::SMEM_BYTES);
+    if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(wide, smem=%d): %s", wide::SMEM_BYTES, cudaGetErrorString(e));
+    cudaFuncAttributes fa;
+    e = cudaFuncGetAttributes(&fa, (const void*)f);
+    if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncGetAttributes(wide): %s", cudaGetErrorString(e));
+    p->fn_wide = f;
+    p->wide = true; p->gmem = true; p->threads = wide_threads; p->n_wacc = 0;
+    p->smem_bytes = wide::SMEM_BYTES; p->regs = fa.numRegs;
+    return PINN_OK;
+}
+
+extern "C" int pinn_plan_create(const PinnSpec* s, int device, PinnPlan** out) {
+    if (!s || !out) return fail(PINN_E_INVALID, "null argument");
+    std::unique_ptr<PinnPlan> p(new (std::nothrow) PinnPlan());
+    if (!p) return fail(PINN_E_INVALID, "out of memory");
     {
-        p->fn_small = nullptr; p->small_smem = 0;
-        bool plain = s->nf <= 4 && order < 3;
-        for (int l = 0; l < h.n_layers; ++l) if (h.layer[l].skip_src >= 0 || h.layer[l].post_base >= 0) plain = false;
-        if (plain) {
-            MultiKernelFn f = nullptr;
-            switch (s->nf) {
-                case 0: f = pinn_small_variant_nf0(s->ns); break;
-                case 1: f = pinn_small_variant_nf1(s->ns); break;
-                case 2: f = pinn_small_variant_nf2(s->ns); break;
-                case 3: f = pinn_small_variant_nf3(s->ns); break;
-                case 4: f = pinn_small_variant_nf4(s->ns); break;
-            }
-            const int bytes = pinn::small::make_layout(h).total * 4;
-            cudaFuncAttributes fs;
-            if (f && cudaFuncGetAttributes(&fs, (const void*)f) == cudaSuccess && bytes <= p->smem_optin - (int)fs.sharedSizeBytes - 64 &&
-                cudaFuncSetAttribute((const void*)f, cudaFuncAttributeMaxDynamicSharedMemorySize, p->smem_optin - (int)fs.sharedSizeBytes) == cudaSuccess) {
-                p->fn_small = f; p->small_smem = bytes;
-            }
-            (void)cudaGetLastError();
-        }
+        char msg[256];
+        const int rc = build_dev_plan(s, p->h, p->fwd_rows, p->fwd_row_scr, msg, sizeof(msg));
+        if (rc) return fail(rc, "%s", msg);
     }
+    // orders 3 / 4 take whole jets per direction (pinn_hi_kernel.cuh), one kernel per (nf, order); their plans have ns = 0
+    const int order = spec_order(s);
+    p->ks = kernels(p->h.nf, p->h.ns, order);
+    if (!p->ks && order >= 3)
+        return fail(PINN_E_UNSUPPORTED, "no kernel for derivative order %d with %d directions", order, s->nf);
+    if (!p->ks)
+        return fail(PINN_E_UNSUPPORTED, "no kernel variant for nf=%d ns=%d%s", s->nf, s->ns,
+                    s->nf > 4 ? " (more than 4 derivative directions: every direction must carry its second derivative, ns = nf)" : "");
+    // a set with the general global-memory form only serves plain plans with it
+    const int gen = p->h.general ? 1 : 0;
+    p->fn_smem = p->ks->step[gen][0];
+    p->fn_gmem = p->ks->step[gen][1] ? p->ks->step[gen][1] : p->ks->step[1][1];
+    p->spec = *s;
+    p->device = device;
 
-    // ---- wide networks: the tensor-core tile kernel takes the step (PINN_FORCE_KERNEL=thread|wide overrides) ----
-    {
-        p->wide = false; p->fn_wide = nullptr; p->wide_ctas = p->sm_count;
-        int mw = 0;
-        const char* fk = getenv("PINN_FORCE_KERNEL");
-        const bool eligible = order < 3 && wide_eligible(h, &mw);
-        // the tile kernel wins from 64-wide layers with many jet channels on (H100 80GB HBM3 at 700 W, cfg5: 21.1 ms
-        // vs 32.3 ms per step); for narrower networks the per (unit, channel) operand handling costs as much as the
-        // FMA row it replaces, and the CUDA-core kernel keeps them
-        bool want = eligible && mw >= 48 && (1 + s->nf + s->ns) >= 5;
-        if (fk && !strcmp(fk, "thread")) want = false;
-        if (fk && !strcmp(fk, "wide")) {
-            if (!eligible) { delete p; return fail(PINN_E_UNSUPPORTED, "PINN_FORCE_KERNEL=wide: this network is outside what the tile kernel covers"); }
-            want = true;
-        }
-        int wide_threads = 512;                     // four threads per point; PINN_WIDE_THREADS=256: two (experiments)
-        { const char* wt = getenv("PINN_WIDE_THREADS"); if (wt && atoi(wt) == 256) wide_threads = 256; }
-        if (want) p->fn_wide = find_wide_variant(s->nf, s->ns, wide_threads);
-        if (want && p->fn_wide) {
-            e = cudaFuncSetAttribute((const void*)p->fn_wide, cudaFuncAttributeMaxDynamicSharedMemorySize, pinn::wide::SMEM_BYTES);
-            if (e != cudaSuccess) { delete p; return fail(PINN_E_CUDA, "cudaFuncSetAttribute(wide, smem=%d): %s", pinn::wide::SMEM_BYTES, cudaGetErrorString(e)); }
-            e = cudaFuncGetAttributes(&fa, (const void*)p->fn_wide);
-            if (e != cudaSuccess) { delete p; return fail(PINN_E_CUDA, "cudaFuncGetAttributes(wide): %s", cudaGetErrorString(e)); }
-            p->wide = true; p->gmem = true; p->threads = wide_threads; p->n_wacc = 0;
-            p->wide_ctas = p->sm_count;
-            p->smem_bytes = pinn::wide::SMEM_BYTES; p->regs = fa.numRegs;
-        }
-    }
+    cudaError_t e = cudaSetDevice(device);
+    if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaSetDevice(%d): %s", device, cudaGetErrorString(e));
+    cudaDeviceProp prop;
+    e = cudaGetDeviceProperties(&prop, device);
+    if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaGetDeviceProperties: %s", cudaGetErrorString(e));
+    if (prop.major != 9 || prop.minor != 0) return fail(PINN_E_UNSUPPORTED, "device sm_%d%d: this library is built for sm_90a only", prop.major, prop.minor);
+    p->sm_count = prop.multiProcessorCount;
+    p->smem_optin = (int)prop.sharedMemPerBlockOptin;
 
-    *out = p;
+    if (int rc = place_step_kernel(p.get())) return rc;
+    if (int rc = place_forward_kernel(p.get())) return rc;
+    place_multi_kernel(p.get());
+    place_small_kernel(p.get());
+    if (int rc = place_wide_kernel(p.get(), order)) return rc;
+    *out = p.release();
     return PINN_OK;
 }
 

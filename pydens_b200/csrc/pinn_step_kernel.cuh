@@ -1,6 +1,6 @@
 // pinn_step_kernel.cuh — the fused fit-step kernel template and its shared-memory staging helpers.
-// Included by pinn_kernels.cu (host API, forward/sampling kernels) and by the per-NF translation
-// units pinn_variants_nf*.cu, which only instantiate step_kernel so the build can run in parallel.
+// Included by pinn_kernels.cu (host API, forward/sampling kernels) and by the build units of
+// pinn_instances.cu, which instantiate the kernels so the build can run in parallel.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -454,13 +454,9 @@ __global__ void __launch_bounds__(MAXT, 1) step_kernel(const __grid_constant__ D
             for (int k = 0; k < P.total; ++k) st[k * RS] = __ldg(src + k);
         } else {
             const uint64_t gidx = a.point_offset + (uint64_t)pe;
-            const uint32_t c3 = (uint32_t)(((step >> 32) & 0xffffu) << 16);
-            Philox4 b0 = philox4x32_10((uint32_t)gidx, (uint32_t)(gidx >> 32), (uint32_t)step, c3,
-                                       (uint32_t)a.seed, (uint32_t)(a.seed >> 32));
+            Philox4 b0 = philox_block(gidx, step, a.seed, 0u);
             Philox4 b1 = b0;
-            if (P.total > 4)
-                b1 = philox4x32_10((uint32_t)gidx, (uint32_t)(gidx >> 32), (uint32_t)step, c3 | 1u,
-                                   (uint32_t)a.seed, (uint32_t)(a.seed >> 32));
+            if (P.total > 4) b1 = philox_block(gidx, step, a.seed, 1u);
             for (int k = 0; k < P.total; ++k) st[k * RS] = sample_column(P.cols[k], k, gidx, step, a.seed, b0, b1);
         }
         float r = point_step<NF, NS, JF, GEN>(P, sw, a.params, st, RS, valid, a.inv_n, sink, part);
@@ -568,13 +564,9 @@ __global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_consta
                 for (int k = 0; k < P.total; ++k) st[k * RS] = __ldg(src + k);
             } else {
                 const uint64_t gidx = (uint64_t)pe;
-                const uint32_t c3 = (uint32_t)(((step >> 32) & 0xffffu) << 16);
-                Philox4 b0 = philox4x32_10((uint32_t)gidx, (uint32_t)(gidx >> 32), (uint32_t)step, c3,
-                                           (uint32_t)a.seed, (uint32_t)(a.seed >> 32));
+                Philox4 b0 = philox_block(gidx, step, a.seed, 0u);
                 Philox4 b1 = b0;
-                if (P.total > 4)
-                    b1 = philox4x32_10((uint32_t)gidx, (uint32_t)(gidx >> 32), (uint32_t)step, c3 | 1u,
-                                       (uint32_t)a.seed, (uint32_t)(a.seed >> 32));
+                if (P.total > 4) b1 = philox_block(gidx, step, a.seed, 1u);
                 for (int k = 0; k < P.total; ++k) st[k * RS] = sample_column(P.cols[k], k, gidx, step, a.seed, b0, b1);
             }
             point_step<NF, NS, JF, true>(P, sw, flat, st, RS, valid, a.inv_n, sink, part);
@@ -639,13 +631,24 @@ typedef void (*MultiKernelFn)(const DevPlan, const MultiArgs);
 
 typedef void (*StepKernelFn)(const DevPlan, const StepArgs);
 
-struct Variant {
-    int nf, ns;
-    StepKernelFn smem_fn, gmem_fn;           // plain problems (no residual wiring / oblique directions / IC variables)
-    StepKernelFn smem_gen_fn, gmem_gen_fn;   // everything
-    MultiKernelFn multi_fn;                  // persistent multi-step kernel (general variant, smem-resident)
-    int maxt;
+// Every kernel instantiation of one jet set: (nf, ns) for second-order problems, (nf, order) for orders 3 / 4.
+// The build units of pinn_instances.cu fill the sets during static initialisation; a null entry has no instantiation.
+struct KernelSet {
+    StepKernelFn step[2][2];                 // step_kernel [GEN][GMEM]; GEN = 0: plain problems (no residual wiring /
+                                             // oblique directions / IC variables / z-stored activations), 1: everything.
+                                             // Five / six directions and orders 3 / 4 have step[1][1] only (orders 3 / 4:
+                                             // hi_step_kernel), which serves plain plans too.
+    MultiKernelFn multi;                     // persistent multi-step kernel (general form, smem-resident)
+    MultiKernelFn small;                     // tiny-batch cluster kernel (pinn_small_kernel.cuh)
+    StepKernelFn wide[2];                    // tensor-core tile kernel (pinn_wide_kernel.cuh), [0]: 512, [1]: 256 threads
+    int maxt;                                // threads per CTA the step kernels are compiled for
 };
+
+// The set of a jet set, or nullptr when none was built: 0 <= ns <= nf <= PINN_MAX_DIRS for order 2; 1 <= nf <= 4 and
+// ns = 0 for orders 3 / 4 (their plans carry no second-order channels).  Defined in pinn_kernels.cu.
+const KernelSet* kernels(int nf, int ns, int order);
+// The writable entry of a jet set, for the build units' static initialisers (same key, not range-checked).
+KernelSet& kernel_slot(int nf, int ns, int order);
 
 template <int NF, int NS>
 struct VariantCfg {
@@ -654,37 +657,4 @@ struct VariantCfg {
     static constexpr int JF = 16;
 };
 
-// `gen` selects which half of the function table this translation unit instantiates (the other half is
-// filled by its sibling unit), so that the two halves compile in parallel.
-template <int NF, int NS, bool GEN>
-static Variant make_variant() {
-    using Cfg = VariantCfg<NF, NS>;
-    Variant v;
-    v.nf = NF; v.ns = NS;
-    v.smem_fn = v.gmem_fn = v.smem_gen_fn = v.gmem_gen_fn = nullptr;
-    v.multi_fn = nullptr;
-    if (GEN) {
-        v.multi_fn = multi_step_kernel<NF, NS, Cfg::MAXT, Cfg::JF>;
-        v.smem_gen_fn = step_kernel<NF, NS, false, Cfg::MAXT, Cfg::JF, GEN>;
-        v.gmem_gen_fn = step_kernel<NF, NS, true, Cfg::MAXT, Cfg::JF, GEN>;
-    } else {
-        v.smem_fn = step_kernel<NF, NS, false, Cfg::MAXT, Cfg::JF, GEN>;
-        v.gmem_fn = step_kernel<NF, NS, true, Cfg::MAXT, Cfg::JF, GEN>;
-    }
-    v.maxt = Cfg::MAXT;
-    return v;
-}
-
 }  // namespace pinn
-
-// one lookup function per NF, each defined in its own translation unit
-const pinn::Variant* pinn_variants_nf0(int ns);
-const pinn::Variant* pinn_variants_nf1(int ns);
-const pinn::Variant* pinn_variants_nf2(int ns);
-const pinn::Variant* pinn_variants_nf3(int ns);
-const pinn::Variant* pinn_variants_nf4(int ns);
-const pinn::Variant* pinn_variants_gen_nf0(int ns);
-const pinn::Variant* pinn_variants_gen_nf1(int ns);
-const pinn::Variant* pinn_variants_gen_nf2(int ns);
-const pinn::Variant* pinn_variants_gen_nf3(int ns);
-const pinn::Variant* pinn_variants_gen_nf4(int ns);

@@ -363,13 +363,9 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
             for (int k = 0; k < PINN_MAX_DIMS; ++k) if (k < P.total) x[k] = __ldg(src + k);
         } else {
             const uint64_t gidx = a.point_offset + (uint64_t)pe;
-            const uint32_t c3 = (uint32_t)(((step >> 32) & 0xffffu) << 16);
-            Philox4 b0 = philox4x32_10((uint32_t)gidx, (uint32_t)(gidx >> 32), (uint32_t)step, c3,
-                                       (uint32_t)a.seed, (uint32_t)(a.seed >> 32));
+            Philox4 b0 = philox_block(gidx, step, a.seed, 0u);
             Philox4 b1 = b0;
-            if (P.total > 4)
-                b1 = philox4x32_10((uint32_t)gidx, (uint32_t)(gidx >> 32), (uint32_t)step, c3 | 1u,
-                                   (uint32_t)a.seed, (uint32_t)(a.seed >> 32));
+            if (P.total > 4) b1 = philox_block(gidx, step, a.seed, 1u);
 #pragma unroll
             for (int k = 0; k < PINN_MAX_DIMS; ++k) if (k < P.total) x[k] = sample_column(P.cols[k], k, gidx, step, a.seed, b0, b1);
         }

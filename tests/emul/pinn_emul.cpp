@@ -127,13 +127,9 @@ extern "C" void emul_sample(const PinnColumn* cols, int total, unsigned long lon
                             unsigned long long point_offset, long long n, float* out) {
     for (long long p = 0; p < n; ++p) {
         const uint64_t gidx = point_offset + (uint64_t)p;
-        const uint32_t c3 = (uint32_t)(((step >> 32) & 0xffffu) << 16);
-        Philox4 b0 = philox4x32_10((uint32_t)gidx, (uint32_t)(gidx >> 32), (uint32_t)step, c3, (uint32_t)seed,
-                                   (uint32_t)(seed >> 32));
+        Philox4 b0 = philox_block(gidx, step, seed, 0u);
         Philox4 b1 = b0;
-        if (total > 4)
-            b1 = philox4x32_10((uint32_t)gidx, (uint32_t)(gidx >> 32), (uint32_t)step, c3 | 1u, (uint32_t)seed,
-                               (uint32_t)(seed >> 32));
+        if (total > 4) b1 = philox_block(gidx, step, seed, 1u);
         for (int k = 0; k < total; ++k) out[p * total + k] = sample_column(cols[k], k, gidx, step, seed, b0, b1);
     }
 }

@@ -72,35 +72,56 @@ def test_library_is_sm90a_and_stages_weights_with_tma():
     assert 'LDS.128' in out                                 # broadcast 128-bit weight loads
 
 
-def test_variant_tables_point_at_the_right_kernel_instantiations():
-    """ The step_kernel instantiations live in several translation units (one per NF, the heavy general ones split
-    by NS); the host dispatch tables must hand out exactly step_kernel<NF, NS, GMEM, MAXT, 16, GEN> for every
-    (NF, NS).  Checked on the host against the exported kernel stubs — no GPU needed. """
-    import ctypes as C
+def test_kernel_table_points_at_the_right_kernel_instantiations():
+    """ The kernel instantiations live in many build units that fill one table at load time; its lookup
+    pinn::kernels(nf, ns, order) must hand out exactly step_kernel<NF, NS, GMEM, MAXT, 16, GEN> and the
+    multi-step, tile and small-batch kernels of every (NF, NS), the five / six direction kernels and
+    hi_step_kernel<NF, K> of orders 3 / 4, and nothing for keys outside those.  Checked on the host against
+    the exported kernel stubs — no GPU needed. """
     lib = C.CDLL(_native.LIB_PATH)
 
-    class Variant(C.Structure):
-        _fields_ = [('nf', C.c_int), ('ns', C.c_int), ('smem_fn', C.c_void_p), ('gmem_fn', C.c_void_p),
-                    ('smem_gen_fn', C.c_void_p), ('gmem_gen_fn', C.c_void_p), ('multi_fn', C.c_void_p), ('maxt', C.c_int)]
+    class KernelSet(C.Structure):
+        _fields_ = [('step', (C.c_void_p * 2) * 2), ('multi', C.c_void_p), ('small', C.c_void_p),
+                    ('wide', C.c_void_p * 2), ('maxt', C.c_int)]
 
-    def stub(nf, ns, gmem, maxt, gen):
-        name = '_ZN4pinn11step_kernelILi%dELi%dELb%dELi%dELi16ELb%dEEEvNS_7DevPlanENS_8StepArgsE' % (nf, ns, gmem, maxt, gen)
+    kernels = lib._ZN4pinn7kernelsEiii
+    kernels.restype = C.POINTER(KernelSet)
+    kernels.argtypes = [C.c_int, C.c_int, C.c_int]
+
+    def addr(name):
         return C.cast(getattr(lib, name), C.c_void_p).value
 
+    def step(nf, ns, gmem, maxt, gen):
+        return addr('_ZN4pinn11step_kernelILi%dELi%dELb%dELi%dELi16ELb%dEEEvNS_7DevPlanENS_8StepArgsE' % (nf, ns, gmem, maxt, gen))
+
     for nf in range(5):
-        for gen in (0, 1):
-            fn = getattr(lib, '_Z%dpinn_variants_%snf%di' % (17 if not gen else 21, 'gen_' if gen else '', nf))
-            fn.restype = C.POINTER(Variant)
-            fn.argtypes = [C.c_int]
-            for ns in range(nf + 1):
-                v = fn(ns).contents
-                maxt = 512 if 1 + nf + ns <= 3 else 256
-                assert (v.nf, v.ns, v.maxt) == (nf, ns, maxt)
-                smem, gmem = (v.smem_gen_fn, v.gmem_gen_fn) if gen else (v.smem_fn, v.gmem_fn)
-                assert smem == stub(nf, ns, 0, maxt, gen) and gmem == stub(nf, ns, 1, maxt, gen), (nf, ns, gen)
-                other = (v.smem_fn, v.gmem_fn) if gen else (v.smem_gen_fn, v.gmem_gen_fn)
-                assert other == (None, None)           # the sibling unit fills the other half (merged at plan creation)
-                # the persistent multi-step kernel rides in the general half
-                mname = '_ZN4pinn17multi_step_kernelILi%dELi%dELi%dELi16EEEvNS_7DevPlanENS_9MultiArgsE' % (nf, ns, maxt)
-                assert v.multi_fn == (C.cast(getattr(lib, mname), C.c_void_p).value if gen else None)
-            assert not fn(nf + 1) and not fn(-1)
+        for ns in range(nf + 1):
+            k = kernels(nf, ns, 2).contents
+            maxt = 512 if 1 + nf + ns <= 3 else 256
+            assert k.maxt == maxt
+            for gen in (0, 1):
+                assert [k.step[gen][0], k.step[gen][1]] == [step(nf, ns, 0, maxt, gen), step(nf, ns, 1, maxt, gen)], (nf, ns, gen)
+            assert k.multi == addr('_ZN4pinn17multi_step_kernelILi%dELi%dELi%dELi16EEEvNS_7DevPlanENS_9MultiArgsE' % (nf, ns, maxt))
+            assert k.small == addr('_ZN4pinn5small17small_step_kernelILi%dELi%dEEEvNS_7DevPlanENS_9MultiArgsE' % (nf, ns))
+            assert list(k.wide) == [addr('_ZN4pinn4wide16wide_step_kernelILi%dELi%dELi%dEEEvNS_7DevPlanENS_8StepArgsE' % (nf, ns, t))
+                                    for t in (512, 256)], (nf, ns)
+        for order in (3, 4):
+            k = kernels(nf, 0, order)
+            if nf == 0:
+                assert not k
+                continue
+            k = k.contents
+            assert k.step[1][1] == addr('_ZN4pinn2hi14hi_step_kernelILi%dELi%dEEEvNS_7DevPlanENS_8StepArgsE' % (nf, order))
+            assert (k.step[0][0], k.step[0][1], k.step[1][0], k.multi, k.small, k.maxt) == (None, None, None, None, None, 256)
+            assert list(k.wide) == [None, None]
+            assert not kernels(nf, 1, order)
+    for nf in (5, 6):
+        k = kernels(nf, nf, 2).contents
+        assert k.step[1][1] == step(nf, nf, 1, 256, 1) and k.maxt == 256
+        assert (k.step[0][0], k.step[0][1], k.step[1][0], k.multi, k.small) == (None, None, None, None, None)
+        assert list(k.wide) == [None, None]
+        for ns in range(nf):
+            assert not kernels(nf, ns, 2)
+        assert not kernels(nf, 0, 3) and not kernels(nf, 0, 4)
+    for key in [(0, 1, 2), (4, 5, 2), (4, -1, 2), (-1, 0, 2), (7, 7, 2), (2, 0, 1), (2, 0, 5), (1, 0, 0)]:
+        assert not kernels(*key), key
