@@ -847,33 +847,35 @@ PINN_HD void act_adjoint2(const ActC& k, const float2 (&pre)[1 + NF + NS], const
 }
 
 #if defined(__CUDA_ARCH__)
+// One stage of warp_transpose_reduce at lane distance S.  S is a template parameter so that every index
+// into v is a compile-time constant and v stays in registers; the selects pick values, not addresses.
+//   S >= NV: every entry is summed with the partner lane's copy of it;
+//   S <  NV: the lower half of the lanes keeps entries [0, S), the upper half keeps [S, 2S) and moves them
+//            down to [0, S); each sends the other half and adds what the partner sent.
+template <int S, int NV>
+__device__ __forceinline__ void warp_transpose_stage(float (&v)[NV], int lane) {
+    if constexpr (S >= NV) {
+#pragma unroll
+        for (int i = 0; i < NV; ++i) v[i] += __shfl_xor_sync(0xffffffffu, v[i], S);
+    } else {
+        const bool up = (lane & S) != 0;
+#pragma unroll
+        for (int i = 0; i < S; ++i) {
+            const float lo = v[i], hi = v[i + S];
+            const float send = up ? lo : hi;
+            const float keep = up ? hi : lo;
+            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, S);
+        }
+    }
+    if constexpr (S > 1) warp_transpose_stage<S / 2, NV>(v, lane);
+}
+
 // Sum NV per-lane values over the 32 lanes of a warp with a transposing butterfly: on return the
 // lane with (lane % NV) == e holds the total of entry e.  31 shuffles for NV == 32.
 template <int NV>
 __device__ __forceinline__ float warp_transpose_reduce(float (&v)[NV], int lane) {
-#pragma unroll
-    for (int s = 16; s >= NV; s >>= 1) {
-#pragma unroll
-        for (int i = 0; i < NV; ++i) v[i] += __shfl_xor_sync(0xffffffffu, v[i], s);
-    }
-#pragma unroll
-    for (int s = (NV / 2 < 16 ? NV / 2 : 16); s >= 1; s >>= 1) {
-        bool up = (lane & s) != 0;
-        if (s >= 2) {                                     // two exchanges per packed add
-#pragma unroll
-            for (int i = 0; i < s; i += 2) {
-                float send0 = up ? v[i] : v[i + s], send1 = up ? v[i + 1] : v[i + 1 + s];
-                float2 keep = make_float2(up ? v[i + s] : v[i], up ? v[i + 1 + s] : v[i + 1]);
-                float2 got = make_float2(__shfl_xor_sync(0xffffffffu, send0, s), __shfl_xor_sync(0xffffffffu, send1, s));
-                keep = make_float2(keep.x + got.x, keep.y + got.y);
-                v[i] = keep.x; v[i + 1] = keep.y;
-            }
-        } else {
-            float send = up ? v[0] : v[1];
-            float keep = up ? v[1] : v[0];
-            v[0] = keep + __shfl_xor_sync(0xffffffffu, send, 1);
-        }
-    }
+    static_assert(NV >= 1 && NV <= 32 && (NV & (NV - 1)) == 0, "NV must be a power of two up to 32");
+    warp_transpose_stage<16, NV>(v, lane);
     return v[0];
 }
 #endif
