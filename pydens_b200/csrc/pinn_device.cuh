@@ -895,25 +895,20 @@ PINN_HD void emit_entries(float (&v)[NV], AddFn&& add) {
 }
 
 struct GradSink {
-    float* wacc;        // accumulator in params layout (+ loss slot) for this warp / CTA
-    bool atomic;        // true when several warps share one accumulator
+    float* wacc;        // this warp's own accumulator in params layout (+ loss slot): no other warp writes it
     int dump;           // index of a scratch slot of the accumulator that swallows masked-off entries
-    // add `val` at `idx` when `valid`; branch-free when the accumulator is private to the warp
+#if !defined(__CUDACC__)
+    bool atomic;        // read by nothing: the host emulation of tests/emul (a plain C++ build) still clears it
+#endif
+    // add `val` at `idx` when `valid`, branch-free
     PINN_HD void add_if(bool valid, int idx, float val) const {
 #if defined(__CUDA_ARCH__)
-        if (atomic) { if (valid) atomicAdd(wacc + idx, val); }
-        else { const int i = valid ? idx : dump; wacc[i] += val; }
+        const int i = valid ? idx : dump; wacc[i] += val;
 #else
         if (valid) wacc[idx] += val;
 #endif
     }
-    PINN_HD void add(int idx, float val) const {
-#if defined(__CUDA_ARCH__)
-        if (atomic) atomicAdd(wacc + idx, val); else wacc[idx] += val;
-#else
-        wacc[idx] += val;
-#endif
-    }
+    PINN_HD void add(int idx, float val) const { wacc[idx] += val; }
 };
 
 // Bias gradients of a layer on their own: for layers whose input width is a multiple of the reduction block

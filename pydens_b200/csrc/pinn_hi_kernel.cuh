@@ -17,18 +17,15 @@ __global__ void __launch_bounds__(256, 1) hi_step_kernel(const __grid_constant__
     extern __shared__ __align__(16) float smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
     const int n_out_floats = P.n_params + 4;
-    const SmemLayout SL = smem_layout(P.weights_floats, n_out_floats, a.n_wacc, P.n_params);
+    const SmemLayout SL = smem_layout(P.weights_floats, n_out_floats, a.wacc ? 0 : nwarps, P.n_params);
     pdl_wait();
     pdl_launch_dependents();
     stage_weights(smem, SL, P, a.params);
     const float* sw = smem + SL.weights_f;
-    float* wacc_all = smem + SL.wacc_f;
-    for (int i = tid; i < n_out_floats * a.n_wacc; i += blockDim.x) wacc_all[i] = 0.0f;
-    __syncthreads();
+    float* wacc_all = warp_accumulators(a, smem, SL, n_out_floats, nwarps);
 
     GradSink sink;
-    sink.atomic = (a.n_wacc == 1 && nwarps > 1);
-    sink.wacc = wacc_all + (a.n_wacc == 1 ? 0 : warp * n_out_floats);
+    sink.wacc = wacc_all + warp * n_out_floats;
     sink.dump = P.n_params + 2;
 
     const long long gw = (long long)blockIdx.x * nwarps + warp;
@@ -75,12 +72,7 @@ __global__ void __launch_bounds__(256, 1) hi_step_kernel(const __grid_constant__
     }
     __syncthreads();
 
-    float* mine = a.partials + (size_t)blockIdx.x * n_out_floats;
-    for (int i = tid; i < n_out_floats; i += blockDim.x) {
-        float s = 0.0f;
-        for (int w = 0; w < a.n_wacc; ++w) s += wacc_all[w * n_out_floats + i];
-        mine[i] = s;
-    }
+    cta_partial(a, wacc_all, n_out_floats, nwarps);
     finish_grid(a, n_out_floats);
 }
 

@@ -138,7 +138,7 @@ struct PinnPlan {
     bool wide;                               // the tensor-core tile kernel runs the step
     StepKernelFn fn_wide;
     MultiKernelFn fn_multi;                  // persistent multi-step kernel, or nullptr when it does not fit
-    int multi_threads, multi_nwacc, multi_smem;
+    int multi_threads, multi_smem;
     MultiKernelFn fn_small;                  // tiny-batch (<= 128 points) variant, or nullptr
     int small_smem;
     int wide_ctas;                           // CTAs the tile kernel runs on (<= sm_count)
@@ -148,7 +148,8 @@ struct PinnPlan {
     int smem_optin;
     // step kernel launch config
     bool gmem;
-    int threads, n_wacc, smem_bytes, regs;
+    bool wacc_gmem;                          // the per-warp gradient accumulators live in the workspace, not in smem
+    int threads, smem_bytes, regs;
     // forward kernel launch config
     bool fwd_gmem;
     int fwd_threads, fwd_smem_bytes, fwd_rows, fwd_row_scr;
@@ -179,8 +180,8 @@ static int storage_floats(const DevPlan& h, int rows, int nw) {
     return rows * RS * nw > h.n_params ? rows * RS * nw : h.n_params;
 }
 
-// Thread kernel: per-point state in shared memory at the largest warp count that fits (per-warp accumulators when
-// they fit too, else one shared accumulator with atomics), or in the global spill area.
+// Thread kernel: per-point state in shared memory at the largest warp count that fits, or in the global spill area.
+// Every warp has a gradient accumulator of its own: in shared memory when it fits there too, else in the workspace.
 static int place_step_kernel(PinnPlan* p) {
     const DevPlan& h = p->h;
     const int n_out_floats = h.n_params + 4;
@@ -191,10 +192,10 @@ static int place_step_kernel(PinnPlan* p) {
     p->regs = fa.numRegs;
     const int max_nw = max_warps(fa, p->ks->maxt);
     const int budget = p->smem_optin - (int)fa.sharedSizeBytes - 64;
-    int best_nw = 0, best_nwacc = 0;
+    int best_nw = 0, best_nwacc = 0;                 // best_nwacc: accumulators in smem (best_nw), or 0 (workspace)
     for (int nw = max_nw; nw >= 1 && !best_nw; --nw) {
         for (int pass = 0; pass < 2 && !best_nw; ++pass) {
-            int nwacc = pass == 0 ? nw : 1;
+            int nwacc = pass == 0 ? nw : 0;
             SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, nwacc, storage_floats(h, h.rows_total, nw));
             if (SL.total_f * 4 <= budget) { best_nw = nw; best_nwacc = nwacc; }
         }
@@ -206,11 +207,11 @@ static int place_step_kernel(PinnPlan* p) {
     if (force && !strcmp(force, "gmem")) use_smem = false;
     if (!has_smem_form) use_smem = false;
     if (use_smem) {
-        p->gmem = false; p->threads = best_nw * 32; p->n_wacc = best_nwacc;
+        p->gmem = false; p->threads = best_nw * 32; p->wacc_gmem = best_nwacc == 0;
         SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, best_nwacc, storage_floats(h, h.rows_total, best_nw));
         p->smem_bytes = SL.total_f * 4;
     } else {
-        // activations spill to a global workspace; accumulators: per warp if they fit, else shared
+        // activations spill to a global workspace; accumulators: in smem if they fit, else in the workspace too
         e = cudaFuncGetAttributes(&fa, (const void*)p->fn_gmem);
         if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncGetAttributes: %s", cudaGetErrorString(e));
         p->regs = fa.numRegs;
@@ -218,9 +219,9 @@ static int place_step_kernel(PinnPlan* p) {
         { const char* e2 = getenv("PINN_GMEM_WARPS"); if (e2 && atoi(e2) >= 1 && atoi(e2) <= nw) nw = atoi(e2); }   // experiments
         int nwacc = nw;
         SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, nwacc, h.n_params);
-        if (SL.total_f * 4 > budget) { nwacc = 1; SL = smem_layout(h.weights_floats, n_out_floats, 1, h.n_params); }
+        if (SL.total_f * 4 > budget) { nwacc = 0; SL = smem_layout(h.weights_floats, n_out_floats, 0, h.n_params); }
         if (SL.total_f * 4 > budget) return fail(PINN_E_UNSUPPORTED, "network too large: %d B of weights do not fit shared memory", SL.total_f * 4);
-        p->gmem = true; p->threads = nw * 32; p->n_wacc = nwacc; p->smem_bytes = SL.total_f * 4;
+        p->gmem = true; p->threads = nw * 32; p->wacc_gmem = nwacc == 0; p->smem_bytes = SL.total_f * 4;
     }
     e = allow_max_smem((const void*)(p->gmem ? p->fn_gmem : p->fn_smem), p->smem_optin);
     if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(smem=%d): %s", p->smem_bytes, cudaGetErrorString(e));
@@ -244,7 +245,7 @@ static int place_forward_kernel(PinnPlan* p) {
 // Persistent multi-step kernel (small batches): per-point state + parameters + Adam moments in shared memory.  Left
 // out when the jet set has none or the network does not fit.
 static void place_multi_kernel(PinnPlan* p) {
-    p->fn_multi = nullptr; p->multi_threads = 0; p->multi_nwacc = 0; p->multi_smem = 0;
+    p->fn_multi = nullptr; p->multi_threads = 0; p->multi_smem = 0;
     const MultiKernelFn f = p->ks->multi;
     if (!f) return;
     cudaFuncAttributes fm;
@@ -256,7 +257,7 @@ static void place_multi_kernel(PinnPlan* p) {
         for (int nw = max_warps(fm, p->ks->maxt); nw >= 1 && !p->fn_multi; --nw) {
             SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, nw, storage_floats(h, h.rows_total, nw));
             if ((SL.total_f + extra) * 4 <= mbudget) {
-                p->fn_multi = f; p->multi_threads = nw * 32; p->multi_nwacc = nw;
+                p->fn_multi = f; p->multi_threads = nw * 32;
                 p->multi_smem = (SL.total_f + extra) * 4;
             }
         }
@@ -307,7 +308,7 @@ static int place_wide_kernel(PinnPlan* p, int order) {
     e = cudaFuncGetAttributes(&fa, (const void*)f);
     if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncGetAttributes(wide): %s", cudaGetErrorString(e));
     p->fn_wide = f;
-    p->wide = true; p->gmem = true; p->threads = wide_threads; p->n_wacc = 0;
+    p->wide = true; p->gmem = true; p->threads = wide_threads; p->wacc_gmem = false;
     p->smem_bytes = wide::SMEM_BYTES; p->regs = fa.numRegs;
     return PINN_OK;
 }
@@ -368,10 +369,16 @@ static int grid_for(const PinnPlan* p, long long n_points, int threads) {
     return (int)ctas;
 }
 
-// workspace layout: [ticket: 256 B][partials: sm_count x n_out_floats][spill]
+// workspace layout: [ticket: 256 B][partials: sm_count x n_out_floats][accumulators][spill]; the thread kernel's
+// per-warp gradient accumulators (sm_count x warps x n_out_floats) are there only when they do not fit shared memory
 static size_t ws_partials_off() { return 256; }
-static size_t ws_spill_off(const PinnPlan* p) {
+static size_t ws_wacc_off(const PinnPlan* p) {
     size_t b = ws_partials_off() + (size_t)p->sm_count * (p->h.n_params + 4) * sizeof(float);
+    return (b + 255) & ~(size_t)255;
+}
+static size_t ws_spill_off(const PinnPlan* p) {
+    size_t b = ws_wacc_off(p);
+    if (p->wacc_gmem) b += (size_t)p->sm_count * (p->threads / 32) * (p->h.n_params + 4) * sizeof(float);
     return (b + 255) & ~(size_t)255;
 }
 
@@ -625,7 +632,8 @@ static int step_impl(const PinnPlan* cp, const PinnComm* comm, const float* para
     a.ticket = reinterpret_cast<unsigned int*>(workspace);
     a.partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_partials_off());
     a.spill = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_spill_off(p));
-    a.n_wacc = p->n_wacc; a.rows_total = p->h.rows_total;
+    a.wacc = p->wacc_gmem ? reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_wacc_off(p)) : nullptr;
+    a.rows_total = p->h.rows_total;
     a.adam_m = nullptr; a.adam_v = nullptr; a.adam_mask = nullptr; a.adam_steps = nullptr; a.adam_n_steps = 0;
     a.adam_lr = a.adam_beta1 = a.adam_beta2 = a.adam_eps = a.adam_wd = 0.0f;
     a.ring = nullptr; a.ring_len = 1;
@@ -716,7 +724,7 @@ extern "C" int pinn_multi_step(const PinnPlan* cp, float* params, float* exp_avg
     a.n_points = n_points; a.inv_n = 1.0f / (float)n_points; a.k_steps = k_steps;
     a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = weight_decay; a.opt_step0 = opt_step0;
     a.losses_ring = losses_ring; a.ring_len = ring_len;
-    a.n_wacc = p->multi_nwacc; a.rows_total = p->h.rows_total;
+    a.rows_total = p->h.rows_total;
     // batches of at most 128 points: the (point, unit)-parallel kernel (PINN_MULTI_KERNEL=tile forces the other one)
     const char* mk = getenv("PINN_MULTI_KERNEL");
     const bool small_ok = p->fn_small && n_points <= 8 * pinn::small::BP && (n_points <= 256 || !p->fn_multi) &&

@@ -29,7 +29,8 @@ struct StepArgs {
     float* partials;
     unsigned int* ticket;
     float* spill;
-    int n_wacc;                            // accumulator copies in smem: warps per CTA, or 1 (atomics)
+    float* wacc;                           // per-warp gradient accumulators in the workspace [grid][warps][n_out_floats],
+                                           // or nullptr: in shared memory
     int rows_total;
     // in-kernel all-reduce over NVLink peer memory (comm_world == 0: off)
     char* comm_peers[PINN_COMM_MAX_RANKS]; // exchange buffer of every rank, mapped through CUDA IPC
@@ -408,6 +409,26 @@ __device__ __forceinline__ void finish_grid(const StepArgs& a, const int n_out_f
     }
 }
 
+// The gradient accumulators of a step: one per warp, [warps][n_out_floats], zeroed.  In shared memory behind the
+// weights, or, when the placement left no room there (a.wacc set), in this CTA's slice of the workspace.  Every warp
+// adds into its own accumulator only, and cta_partial sums them in warp order: the result does not depend on timing.
+__device__ __forceinline__ float* warp_accumulators(const StepArgs& a, float* smem, const SmemLayout& SL,
+                                                    int n_out_floats, int nwarps) {
+    float* w = a.wacc ? a.wacc + (size_t)blockIdx.x * nwarps * n_out_floats : smem + SL.wacc_f;
+    for (int i = threadIdx.x; i < n_out_floats * nwarps; i += blockDim.x) w[i] = 0.0f;
+    __syncthreads();
+    return w;
+}
+// The CTA's partial [n_out_floats] -> a.partials[blockIdx.x]: the warps' accumulators summed in warp order.
+__device__ __forceinline__ void cta_partial(const StepArgs& a, const float* wacc_all, int n_out_floats, int nwarps) {
+    float* mine = a.partials + (size_t)blockIdx.x * n_out_floats;
+    for (int i = threadIdx.x; i < n_out_floats; i += blockDim.x) {
+        float s = 0.0f;
+        for (int w = 0; w < nwarps; ++w) s += wacc_all[w * n_out_floats + i];
+        mine[i] = s;
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------
 // The fit-step kernel.
 // ---------------------------------------------------------------------------------------------------
@@ -417,19 +438,16 @@ __global__ void __launch_bounds__(MAXT, 1) step_kernel(const __grid_constant__ D
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
 
     const int n_out_floats = P.n_params + 4;
-    const SmemLayout SL = smem_layout(P.weights_floats, n_out_floats, a.n_wacc,
+    const SmemLayout SL = smem_layout(P.weights_floats, n_out_floats, a.wacc ? 0 : nwarps,
                                       GMEM ? P.n_params : max(P.n_params, a.rows_total * RS * nwarps));
     pdl_wait();                                    // the previous step (its parameter update) is complete and visible
     pdl_launch_dependents();                       // the next step's CTAs may take the SMs as ours leave them
     stage_weights(smem, SL, P, a.params);
     const float* sw = smem + SL.weights_f;
-    float* wacc_all = smem + SL.wacc_f;
-    for (int i = tid; i < n_out_floats * a.n_wacc; i += blockDim.x) wacc_all[i] = 0.0f;
-    __syncthreads();
+    float* wacc_all = warp_accumulators(a, smem, SL, n_out_floats, nwarps);
 
     GradSink sink;
-    sink.atomic = (a.n_wacc == 1 && nwarps > 1);
-    sink.wacc = wacc_all + (a.n_wacc == 1 ? 0 : warp * n_out_floats);
+    sink.wacc = wacc_all + warp * n_out_floats;
     sink.dump = P.n_params + 2;                    // spare float behind the loss slot
 
     const long long gw = (long long)blockIdx.x * nwarps + warp;         // global warp id
@@ -480,12 +498,7 @@ __global__ void __launch_bounds__(MAXT, 1) step_kernel(const __grid_constant__ D
     __syncthreads();
 
     // CTA partial -> global, then the last CTA folds all partials in block order
-    float* mine = a.partials + (size_t)blockIdx.x * n_out_floats;
-    for (int i = tid; i < n_out_floats; i += blockDim.x) {
-        float s = 0.0f;
-        for (int w = 0; w < a.n_wacc; ++w) s += wacc_all[w * n_out_floats + i];
-        mine[i] = s;
-    }
+    cta_partial(a, wacc_all, n_out_floats, nwarps);
     finish_grid(a, n_out_floats);
 }
 
@@ -516,7 +529,7 @@ struct MultiArgs {
     float opt_step0;               // optimizer steps taken before this launch
     float* losses_ring;
     long long ring_len;
-    int n_wacc, rows_total;
+    int rows_total;
 };
 
 template <int NF, int NS, int MAXT, int JF>
@@ -525,7 +538,7 @@ __global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_consta
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
     const int n_out_floats = P.n_params + 4;
     const int storage_f = max(P.n_params, a.rows_total * RS * nwarps);
-    const SmemLayout SL = smem_layout(P.weights_floats, n_out_floats, a.n_wacc, storage_f);
+    const SmemLayout SL = smem_layout(P.weights_floats, n_out_floats, nwarps, storage_f);
     // behind the single-step layout: flat parameters, both Adam moments, the folded gradient
     float* flat = smem + SL.total_f;
     float* mom1 = flat + align4(P.n_params);
@@ -540,15 +553,14 @@ __global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_consta
     __syncthreads();
 
     GradSink sink;
-    sink.atomic = (a.n_wacc == 1 && nwarps > 1);
-    sink.wacc = wacc_all + (a.n_wacc == 1 ? 0 : warp * n_out_floats);
+    sink.wacc = wacc_all + warp * n_out_floats;
     sink.dump = P.n_params + 2;
     float* st = smem + SL.storage_f + (size_t)warp * a.rows_total * RS + lane;
     const unsigned long long step0 = *a.step_counter;
     const long long n_tiles = (a.n_points + 31) / 32;
 
     for (int s = 0; s < a.k_steps; ++s) {
-        for (int i = tid; i < n_out_floats * a.n_wacc; i += blockDim.x) wacc_all[i] = 0.0f;
+        for (int i = tid; i < n_out_floats * nwarps; i += blockDim.x) wacc_all[i] = 0.0f;
         __syncthreads();
         const uint64_t step = step0 + (unsigned long long)s;
         PointPartials<NF, NS> part;
@@ -592,7 +604,7 @@ __global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_consta
         const float step_size = a.lr / bc1;
         for (int i = tid; i < n_out_floats; i += blockDim.x) {
             float g = 0.0f;
-            for (int w = 0; w < a.n_wacc; ++w) g += wacc_all[w * n_out_floats + i];
+            for (int w = 0; w < nwarps; ++w) g += wacc_all[w * n_out_floats + i];
             gsum[i] = g;
             if (i < P.n_params && a.mask[i] != 0.0f) {
                 float pv = flat[i];
