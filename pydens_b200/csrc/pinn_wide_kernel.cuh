@@ -1,4 +1,4 @@
-// pinn_wide_kernel.cuh — the fit step for WIDE networks (hidden widths 17..64) on Hopper tensor cores.
+// pinn_wide_kernel.cuh — the fit step for WIDE networks (hidden widths up to 64) on Hopper tensor cores.
 //
 // The thread-per-point kernel (pinn_step_kernel.cuh) runs every matrix product of the step on CUDA cores and has
 // to keep `units x channels` floats of state per point; for a 64-wide network carrying 9 jet channels that is
@@ -7,10 +7,10 @@
 // :107-128, MSE :448, loss.backward() :460) is organised around warp-level tensor-core MMAs (mma.sync m16n8k8 tf32):
 //
 //   * CTA tile = 128 collocation points; 512 threads: thread (p, quarter) owns point p and one quarter of the 64
-//     hidden units, so every per-(point, unit) quantity is thread-private.
+//     hidden units, so every per-(point, unit) quantity is thread-private (256 threads: one half each).
 //   * Every hidden->hidden product, for every jet channel c, is one GEMM  Z_c[128 x 64] = A_c[128 x 64] . W^T
 //     with A_c written row-per-thread into shared memory, W staged [n][k] in shared memory, and Z_c written back to
-//     shared memory, where the thread of each point reads its row.  Every warp computes a 16 x 32 block.  Operands
+//     shared memory, where the thread of each point reads its row.  The 16 x 32 blocks are dealt to the warps.  Operands
 //     are split hi/lo as they are loaded and multiplied as 3xTF32 (lo.hi + hi.lo + hi.hi): fp32 grade — single-pass
 //     TF32 (7e-4 relative) cannot hold the 1e-4 bar.
 //   * The reverse sweep is the same machinery: the data gradient  abar_{h-1} = delta_h . W  is again such a GEMM,
@@ -24,9 +24,10 @@
 //     memory that is written and re-read by the same thread (L2-resident working set), 256 B per (point, channel,
 //     level); the adjoint of a level overwrites the dead slot of the level above.
 //
-// Covered: dense chains 'fa…f' with tanh / sigmoid / identity hidden activations, hidden widths <= 64, up to
-// 7 linear layers, every jet set / ansatz / residual program / sampler the thread kernel covers.  Everything else
-// (residual layouts, sin/softplus/SiLU/GELU) stays on the thread kernel.
+// Covered: dense chains 'fa…f' with tanh / sigmoid / identity hidden activations, any hidden width <= 64, 2 to 6
+// linear layers (MAX_LAYERS), the jet sets NS <= NF <= 4, every ansatz / residual program / sampler the thread kernel
+// covers (tests/test_gpu_tile.py).  Everything else (residual layouts, sin/softplus/SiLU/GELU, wider layers, more
+// layers, orders 3 / 4) stays on the thread kernels.
 #pragma once
 
 #include "pinn_step_kernel.cuh"
@@ -577,8 +578,9 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
                     }
                 }
                 if (h >= 2) {
-                    // warps 0/1: the data gradient, 32 columns each; warps 2/3: the two K halves of the weight
-                    // gradient (and, on the value channel, of the bias gradient)
+                    // every warp takes its share of each GEMM's items: the data gradient (16 x 32 blocks), the
+                    // weight gradient (16 x 16 blocks) and, on the value channel, the bias gradient (dealt from the
+                    // last warp down)
                     sync_issue([&](int w) {
                         gemm_rows(smem, kp, np, w, NT / 32);
                         gemm_wgrad(smem, reinterpret_cast<float*>(smem + S_WACC) + (h - 2) * KW * KW, L.n_out, L.n_in, w, NT / 32);
