@@ -410,7 +410,10 @@ typedef struct PinnPlanInfo {
     int32_t rows_per_point;           /* floats of per-point state kept between fwd/bwd  */
     int64_t flops_per_point;          /* algorithmic 6*C*M (SURVEY.md 8d)                */
     int32_t bytes_per_point;          /* algorithmic 4*(ndims+nparams)                   */
-    int32_t tensor_core;              /* 1: the tensor-core tile kernel for wide networks runs the step (3xTF32),
+    int32_t tensor_core;              /* 1: the tensor-core tile kernel for wide networks runs the step (3xTF32,
+                                            hidden widths <= 64),
+                                         2: its 128-wide class runs it (hidden widths up to 128; networks whose
+                                            weights the thread kernel cannot hold in shared memory),
                                          0: the thread-per-point FP32 kernel                 */
     int32_t small_batch_points;       /* largest batch the cluster (point, unit)-parallel loop kernel takes through
                                          pinn_multi_step (8 CTAs x 128 points), 0: the network does not fit it         */

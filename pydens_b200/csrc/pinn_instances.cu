@@ -10,10 +10,11 @@
 #define PINN_HI_JET 4        // hi_step_kernel, derivatives of order 3 / 4
 #define PINN_WIDE 5          // wide_step_kernel, the tensor-core tile kernel
 #define PINN_SMALL 6         // small_step_kernel, the tiny-batch cluster kernel
+#define PINN_WIDE128 7       // wide_step_kernel of the 128-wide class
 
 #if PINN_UNIT == PINN_HI_JET
 #include "pinn_hi_kernel.cuh"
-#elif PINN_UNIT == PINN_WIDE
+#elif PINN_UNIT == PINN_WIDE || PINN_UNIT == PINN_WIDE128
 #include "pinn_wide_kernel.cuh"
 #elif PINN_UNIT == PINN_SMALL
 #include "pinn_small_kernel.cuh"
@@ -52,6 +53,8 @@ void enter() {
     KernelSet& k = kernel_slot(NF, J, 2);
     k.wide[0] = wide::wide_step_kernel<NF, J, 512>;
     k.wide[1] = wide::wide_step_kernel<NF, J, 256>;
+#elif PINN_UNIT == PINN_WIDE128
+    kernel_slot(NF, J, 2).wide128 = wide::wide128_step_kernel<NF, J>;
 #elif PINN_UNIT == PINN_SMALL
     kernel_slot(NF, J, 2).small = small::small_step_kernel<NF, J>;
 #else

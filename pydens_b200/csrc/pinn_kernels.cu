@@ -66,6 +66,11 @@ __global__ void __launch_bounds__(256, 1) forward_kernel(const __grid_constant__
     }
 }
 
+// The forward-only form of the 128-wide tile kernel (declared in pinn_wide_kernel.cuh).
+__global__ void __launch_bounds__(512, 1) wide::wide128_forward_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
+    wide::wide_step<0, 0, 512, 128, true>(P, a);
+}
+
 // Points the in-kernel sampler produces (for tests / replay).
 struct SampleCols { PinnColumn c[PINN_MAX_DIMS]; int total; };
 
@@ -117,7 +122,8 @@ static int fail(int code, const char* fmt, ...) {
     } while (0)
 
 // The tensor-core tile kernel (pinn_wide_kernel.cuh) covers plain dense chains with polynomial-family activations
-// and hidden widths <= 64; it pays off once the layers are wide enough to be real GEMMs.
+// and hidden widths <= 128, in two width classes (<= 64 and 65..128); it pays off once the layers are wide enough to
+// be real GEMMs.  *max_width: the widest hidden layer.
 static bool wide_eligible(const pinn::DevPlan& h, int* max_width) {
     if (h.n_layers < 2 || h.n_layers > pinn::wide::MAX_LAYERS) return false;
     int mw = 0;
@@ -125,7 +131,7 @@ static bool wide_eligible(const pinn::DevPlan& h, int* max_width) {
         const pinn::DevLayer& L = h.layer[l];
         if (L.skip_src >= 0 || L.post_base >= 0) return false;
         if (L.act != PINN_ACT_NONE && L.act != PINN_ACT_TANH && L.act != PINN_ACT_SIGMOID) return false;
-        if (l + 1 < h.n_layers) { if (L.n_out > pinn::wide::KW) return false; if (L.n_out > mw) mw = L.n_out; }
+        if (l + 1 < h.n_layers) { if (L.n_out > pinn::wide::Tile<128>::KW) return false; if (L.n_out > mw) mw = L.n_out; }
     }
     *max_width = mw;
     return true;
@@ -136,6 +142,7 @@ struct PinnPlan {
     DevPlan h;
     int device;
     bool wide;                               // the tensor-core tile kernel runs the step
+    int wide_kw;                             // its width class: 64 or 128
     StepKernelFn fn_wide;
     MultiKernelFn fn_multi;                  // persistent multi-step kernel, or nullptr when it does not fit
     int multi_threads, multi_smem;
@@ -152,6 +159,7 @@ struct PinnPlan {
     int threads, smem_bytes, regs;
     // forward kernel launch config
     bool fwd_gmem;
+    bool fwd_wide;                           // pinn_forward runs the 128-wide tile kernel's forward-only form
     int fwd_threads, fwd_smem_bytes, fwd_rows, fwd_row_scr;
 };
 
@@ -283,33 +291,49 @@ static void place_small_kernel(PinnPlan* p) {
     (void)cudaGetLastError();
 }
 
-// Wide networks: the tensor-core tile kernel takes the step (PINN_FORCE_KERNEL=thread|wide overrides).
-static int place_wide_kernel(PinnPlan* p, int order) {
-    p->wide = false; p->fn_wide = nullptr; p->wide_ctas = p->sm_count;
+// Wide networks: the tensor-core tile kernel takes the step (PINN_FORCE_KERNEL=thread|wide|wide128 overrides).
+// thread_rc is how the thread kernel's placement (step and forward) went: a network whose weights do not fit its
+// shared memory goes to the 128-wide class when that class covers it; otherwise that failure is the plan's.
+static int place_wide_kernel(PinnPlan* p, int order, int thread_rc) {
+    p->wide = false; p->fn_wide = nullptr; p->wide_ctas = p->sm_count; p->wide_kw = 64; p->fwd_wide = false;
     int mw = 0;
     const char* fk = getenv("PINN_FORCE_KERNEL");
     const bool eligible = order < 3 && wide_eligible(p->h, &mw);
+    const bool eligible128 = eligible && mw > 64 && p->ks->wide128;
     // the tile kernel wins from 64-wide layers with many jet channels on (H100 80GB HBM3 at 700 W, cfg5: 21.1 ms
     // vs 32.3 ms per step); for narrower networks the per (unit, channel) operand handling costs as much as the
-    // FMA row it replaces, and the CUDA-core kernel keeps them
-    bool want = eligible && mw >= 48 && (1 + p->spec.nf + p->spec.ns) >= 5;
+    // FMA row it replaces, and the CUDA-core kernel keeps them.  Networks of 65-128 units the thread kernel holds
+    // stay there: the 128-wide class takes only what the thread kernel refuses.
+    bool want = eligible && mw <= 64 && mw >= 48 && (1 + p->spec.nf + p->spec.ns) >= 5;
+    int kw = 64;
+    if (thread_rc != PINN_OK) { want = eligible128; kw = 128; }
     if (fk && !strcmp(fk, "thread")) want = false;
     if (fk && !strcmp(fk, "wide")) {
-        if (!eligible) return fail(PINN_E_UNSUPPORTED, "PINN_FORCE_KERNEL=wide: this network is outside what the tile kernel covers");
-        want = true;
+        if (!eligible || mw > 64) return fail(PINN_E_UNSUPPORTED, "PINN_FORCE_KERNEL=wide: this network is outside what the tile kernel covers");
+        want = true; kw = 64;
     }
-    int wide_threads = 512;                     // four threads per point; PINN_WIDE_THREADS=256: two (experiments)
-    { const char* wt = getenv("PINN_WIDE_THREADS"); if (wt && atoi(wt) == 256) wide_threads = 256; }
-    const StepKernelFn f = p->ks->wide[wide_threads == 256 ? 1 : 0];
-    if (!want || !f) return PINN_OK;
-    cudaError_t e = cudaFuncSetAttribute((const void*)f, cudaFuncAttributeMaxDynamicSharedMemorySize, wide::SMEM_BYTES);
-    if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(wide, smem=%d): %s", wide::SMEM_BYTES, cudaGetErrorString(e));
+    if (fk && !strcmp(fk, "wide128")) {
+        if (!eligible128) return fail(PINN_E_UNSUPPORTED, "PINN_FORCE_KERNEL=wide128: this network is outside what the 128-wide tile kernel covers");
+        want = true; kw = 128;
+    }
+    int wide_threads = 512;                     // four threads per point; PINN_WIDE_THREADS=256: two (experiments, 64-wide class)
+    { const char* wt = getenv("PINN_WIDE_THREADS"); if (wt && atoi(wt) == 256 && kw == 64) wide_threads = 256; }
+    const StepKernelFn f = kw == 128 ? p->ks->wide128 : p->ks->wide[wide_threads == 256 ? 1 : 0];
+    if (!want || !f || (thread_rc != PINN_OK && kw != 128)) return thread_rc;
+    const int smem = kw == 128 ? wide::Tile<128>::SMEM_BYTES : wide::Tile<64>::SMEM_BYTES;
+    cudaError_t e = cudaFuncSetAttribute((const void*)f, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(wide, smem=%d): %s", smem, cudaGetErrorString(e));
     cudaFuncAttributes fa;
     e = cudaFuncGetAttributes(&fa, (const void*)f);
     if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncGetAttributes(wide): %s", cudaGetErrorString(e));
     p->fn_wide = f;
-    p->wide = true; p->gmem = true; p->threads = wide_threads; p->wacc_gmem = false;
-    p->smem_bytes = wide::SMEM_BYTES; p->regs = fa.numRegs;
+    p->wide = true; p->wide_kw = kw; p->gmem = true; p->threads = wide_threads; p->wacc_gmem = false;
+    p->smem_bytes = smem; p->regs = fa.numRegs;
+    if (thread_rc != PINN_OK) {                 // the forward kernel does not hold this network either
+        e = cudaFuncSetAttribute((const void*)wide::wide128_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(wide forward, smem=%d): %s", smem, cudaGetErrorString(e));
+        p->fwd_wide = true; p->fwd_gmem = false;
+    }
     return PINN_OK;
 }
 
@@ -346,11 +370,14 @@ extern "C" int pinn_plan_create(const PinnSpec* s, int device, PinnPlan** out) {
     p->sm_count = prop.multiProcessorCount;
     p->smem_optin = (int)prop.sharedMemPerBlockOptin;
 
-    if (int rc = place_step_kernel(p.get())) return rc;
-    if (int rc = place_forward_kernel(p.get())) return rc;
+    // the thread kernels (step and forward); a network whose weights do not fit their shared memory can still go to
+    // the 128-wide tile kernel, which stages one layer at a time (place_wide_kernel)
+    int thread_rc = place_step_kernel(p.get());
+    if (thread_rc == PINN_OK) thread_rc = place_forward_kernel(p.get());
+    if (thread_rc != PINN_OK && thread_rc != PINN_E_UNSUPPORTED) return thread_rc;
     place_multi_kernel(p.get());
     place_small_kernel(p.get());
-    if (int rc = place_wide_kernel(p.get(), order)) return rc;
+    if (int rc = place_wide_kernel(p.get(), order, thread_rc)) return rc;
     *out = p.release();
     return PINN_OK;
 }
@@ -369,16 +396,20 @@ static int grid_for(const PinnPlan* p, long long n_points, int threads) {
     return (int)ctas;
 }
 
-// workspace layout: [ticket: 256 B][partials: sm_count x n_out_floats][accumulators][spill]; the thread kernel's
-// per-warp gradient accumulators (sm_count x warps x n_out_floats) are there only when they do not fit shared memory
+// workspace layout: [ticket: 256 B][partials: sm_count x n_out_floats][accumulators][spill]; the accumulators are the
+// thread kernel's per-warp gradient accumulators (sm_count x warps x n_out_floats) when they do not fit shared memory,
+// or the 128-wide tile kernel's hidden->hidden weight gradients (sm_count x 4 x 128 x 128, 256 KB per CTA)
 static size_t ws_partials_off() { return 256; }
 static size_t ws_wacc_off(const PinnPlan* p) {
     size_t b = ws_partials_off() + (size_t)p->sm_count * (p->h.n_params + 4) * sizeof(float);
     return (b + 255) & ~(size_t)255;
 }
+static size_t ws_wacc_bytes(const PinnPlan* p) {
+    if (p->wide) return p->wide_kw == 128 ? (size_t)p->sm_count * wide::Tile<128>::WACC_FLOATS * sizeof(float) : 0;
+    return p->wacc_gmem ? (size_t)p->sm_count * (p->threads / 32) * (p->h.n_params + 4) * sizeof(float) : 0;
+}
 static size_t ws_spill_off(const PinnPlan* p) {
-    size_t b = ws_wacc_off(p);
-    if (p->wacc_gmem) b += (size_t)p->sm_count * (p->threads / 32) * (p->h.n_params + 4) * sizeof(float);
+    size_t b = ws_wacc_off(p) + ws_wacc_bytes(p);
     return (b + 255) & ~(size_t)255;
 }
 
@@ -632,7 +663,7 @@ static int step_impl(const PinnPlan* cp, const PinnComm* comm, const float* para
     a.ticket = reinterpret_cast<unsigned int*>(workspace);
     a.partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_partials_off());
     a.spill = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_spill_off(p));
-    a.wacc = p->wacc_gmem ? reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_wacc_off(p)) : nullptr;
+    a.wacc = ws_wacc_bytes(p) ? reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_wacc_off(p)) : nullptr;
     a.rows_total = p->h.rows_total;
     a.adam_m = nullptr; a.adam_v = nullptr; a.adam_mask = nullptr; a.adam_steps = nullptr; a.adam_n_steps = 0;
     a.adam_lr = a.adam_beta1 = a.adam_beta2 = a.adam_eps = a.adam_wd = 0.0f;
@@ -660,11 +691,12 @@ static int step_impl(const PinnPlan* cp, const PinnComm* comm, const float* para
     a.comm_world = comm ? comm->world : 0;
     for (int r = 0; r < PINN_COMM_MAX_RANKS; ++r) a.comm_peers[r] = comm ? comm->peers[r] : nullptr;
     if (p->wide) {
-        long long tiles = (n_points + pinn::wide::T - 1) / pinn::wide::T;
+        const int T = p->wide_kw == 128 ? wide::Tile<128>::T : wide::Tile<64>::T;
+        long long tiles = (n_points + T - 1) / T;
         int max_ctas = p->wide_ctas;
         { const char* e = getenv("PINN_WIDE_CTAS"); if (e && atoi(e) >= 1 && atoi(e) <= p->sm_count) max_ctas = atoi(e); }   // experiments
         const int grid = (int)(tiles < max_ctas ? tiles : max_ctas);
-        return launch_step(p->fn_wide, grid, p->threads, pinn::wide::SMEM_BYTES, st, plan, a);
+        return launch_step(p->fn_wide, grid, p->threads, p->smem_bytes, st, plan, a);
     }
     const int grid = grid_for(p, n_points, p->threads);
     StepKernelFn fn = p->gmem ? p->fn_gmem : p->fn_smem;
@@ -759,12 +791,20 @@ extern "C" int pinn_forward(const PinnPlan* p, const float* params, const float*
     if (!aligned16(params) || !aligned16(workspace)) return fail(PINN_E_ALIGN, "params / workspace must be 16-byte aligned");
     if (((uintptr_t)points) & 3u) return fail(PINN_E_ALIGN, "points must be 4-byte aligned");
     if (workspace_bytes < pinn_workspace_bytes(p, n_points)) return fail(PINN_E_WORKSPACE, "workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (p->fwd_wide) {                         // u of every point goes to `out` of the step arguments
+        StepArgs w;
+        memset(&w, 0, sizeof(w));
+        w.params = params; w.points = points; w.n_points = n_points; w.out = u_out; w.ring_len = 1;
+        const long long tiles = (n_points + wide::Tile<128>::T - 1) / wide::Tile<128>::T;
+        const int grid = (int)(tiles < p->sm_count ? tiles : p->sm_count);
+        return launch_step(wide::wide128_forward_kernel, grid, 512, wide::Tile<128>::SMEM_BYTES, st, p->h, w);
+    }
     FwdArgs a;
     a.params = params; a.points = points; a.n_points = n_points; a.u_out = u_out;
     a.spill = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_spill_off(p));
     a.rows_total = p->fwd_rows; a.row_scr = p->fwd_row_scr;
     const int grid = grid_for(p, n_points, p->fwd_threads);
-    cudaStream_t st = (cudaStream_t)stream;
     if (p->fwd_gmem) forward_kernel<true><<<grid, p->fwd_threads, p->fwd_smem_bytes, st>>>(p->h, a);
     else             forward_kernel<false><<<grid, p->fwd_threads, p->fwd_smem_bytes, st>>>(p->h, a);
     CUDA_TRY(cudaGetLastError());
@@ -806,7 +846,7 @@ extern "C" int pinn_plan_info(const PinnPlan* p, PinnPlanInfo* info) {
     info->nf = p->h.nf; info->ns = p->h.ns; info->channels = C;
     info->threads_per_cta = p->threads; info->ctas_per_sm = 1;
     info->activations_in_smem = p->gmem ? 0 : 1;
-    info->tensor_core = p->wide ? 1 : 0;
+    info->tensor_core = p->wide ? (p->wide_kw == 128 ? 2 : 1) : 0;
     info->small_batch_points = p->fn_small ? 8 * pinn::small::BP : 0;
     info->smem_bytes = p->smem_bytes; info->regs_per_thread = p->regs; info->sm_count = p->sm_count;
     info->rows_per_point = p->h.rows_total;

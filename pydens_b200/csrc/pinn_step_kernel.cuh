@@ -654,6 +654,7 @@ struct KernelSet {
     MultiKernelFn small;                     // tiny-batch cluster kernel (pinn_small_kernel.cuh)
     StepKernelFn wide[2];                    // tensor-core tile kernel (pinn_wide_kernel.cuh), [0]: 512, [1]: 256 threads
     int maxt;                                // threads per CTA the step kernels are compiled for
+    StepKernelFn wide128;                    // the tile kernel's class for hidden widths up to 128, 512 threads
 };
 
 // The set of a jet set, or nullptr when none was built: 0 <= ns <= nf <= PINN_MAX_DIRS for order 2; 1 <= nf <= 4 and

@@ -1,33 +1,38 @@
-// pinn_wide_kernel.cuh — the fit step for WIDE networks (hidden widths up to 64) on Hopper tensor cores.
+// pinn_wide_kernel.cuh — the fit step for WIDE networks (hidden widths up to 128) on Hopper tensor cores.
 //
 // The thread-per-point kernel (pinn_step_kernel.cuh) runs every matrix product of the step on CUDA cores and has
 // to keep `units x channels` floats of state per point; for a 64-wide network carrying 9 jet channels that is
 // 2 300 floats per point and it does not fit on the SM.  Here the same step (reference pydens/model_torch.py:430-460:
 // forward of ConvBlockModel :170-172 with the nested D() derivatives :174-178 carried as jet channels, ansatz
-// :107-128, MSE :448, loss.backward() :460) is organised around warp-level tensor-core MMAs (mma.sync m16n8k8 tf32):
+// :107-128, MSE :448, loss.backward() :460) is organised around warp-level tensor-core MMAs (mma.sync m16n8k8 tf32).
+// Two width classes share one body (wide_step): KW = 64 (wide_step_kernel) and KW = 128 (wide128_step_kernel, for
+// networks whose weights the thread kernel cannot hold in shared memory); the tile is T = 8192 / KW points.
 //
-//   * CTA tile = 128 collocation points; 512 threads: thread (p, quarter) owns point p and one quarter of the 64
-//     hidden units, so every per-(point, unit) quantity is thread-private (256 threads: one half each).
-//   * Every hidden->hidden product, for every jet channel c, is one GEMM  Z_c[128 x 64] = A_c[128 x 64] . W^T
-//     with A_c written row-per-thread into shared memory, W staged [n][k] in shared memory, and Z_c written back to
-//     shared memory, where the thread of each point reads its row.  The 16 x 32 blocks are dealt to the warps.  Operands
-//     are split hi/lo as they are loaded and multiplied as 3xTF32 (lo.hi + hi.lo + hi.hi): fp32 grade — single-pass
-//     TF32 (7e-4 relative) cannot hold the 1e-4 bar.
+//   * CTA tile = T collocation points (128 or 64); 512 threads: thread (p, part) owns point p and 16 of the KW hidden
+//     units, so every per-(point, unit) quantity is thread-private (KW = 64 at 256 threads: 32 units each).
+//   * Every hidden->hidden product, for every jet channel c, is one GEMM  Z_c[T x KW] = A_c[T x KW] . W^T
+//     with A_c written row-per-thread into shared memory, W staged [n][k] in shared memory (one layer at a time), and
+//     Z_c written back to shared memory, where the thread of each point reads its row.  The 16 x 32 blocks (16 of them
+//     in both classes) are dealt to the warps.  Operands are split hi/lo as they are loaded and multiplied as 3xTF32
+//     (lo.hi + hi.lo + hi.hi): fp32 grade — single-pass TF32 (7e-4 relative) cannot hold the 1e-4 bar.
 //   * The reverse sweep is the same machinery: the data gradient  abar_{h-1} = delta_h . W  is again such a GEMM,
-//     and EVERY reduction over points — weight gradients  Wbar = sum_p delta^T a  (M = 64 output units, N = 64 input
-//     units, K = the 128 points of the tile, both operands read transposed from the same row-per-point buffers),
+//     and EVERY reduction over points — weight gradients  Wbar = sum_p delta^T a  (M = KW output units, N = KW input
+//     units, K = the T points of the tile, both operands read transposed from the same row-per-point buffers),
 //     bias gradients, the first layer's and the output layer's weight gradients (small-N GEMMs against a
-//     [16 x 128] right-hand side) — runs on the tensor cores.  Each accumulator block belongs to one warp, which
-//     adds a tile's product into a shared-memory accumulator that lives for the whole kernel: no shuffles, no
-//     atomics, a fixed summation order.  The accumulators are read out once at the end of the kernel.
+//     [16 x T] right-hand side) — runs on the tensor cores.  Each accumulator block belongs to one warp, which adds a
+//     tile's product into an accumulator that lives for the whole kernel: no shuffles, no atomics, a fixed summation
+//     order.  The accumulators are in shared memory, except the hidden->hidden weight gradients of the 128-wide class
+//     (4 x 64 KB), which are in this CTA's area of the workspace.  They are read out once at the end of the kernel.
 //   * Between the GEMMs the per-point state (a, z_d, z_dd per unit and channel) lives in a per-CTA slab of global
-//     memory that is written and re-read by the same thread (L2-resident working set), 256 B per (point, channel,
+//     memory that is written and re-read by the same thread (L2-resident working set), T x KW floats per (channel,
 //     level); the adjoint of a level overwrites the dead slot of the level above.
+//   * wide128_forward_kernel is the forward-only form of the 128-wide class (pinn_forward): the value channel's
+//     forward sweep and the ansatz, no slab.
 //
-// Covered: dense chains 'fa…f' with tanh / sigmoid / identity hidden activations, any hidden width <= 64, 2 to 6
-// linear layers (MAX_LAYERS), the jet sets NS <= NF <= 4, every ansatz / residual program / sampler the thread kernel
-// covers (tests/test_gpu_tile.py).  Everything else (residual layouts, sin/softplus/SiLU/GELU, wider layers, more
-// layers, orders 3 / 4) stays on the thread kernels.
+// Covered: dense chains 'fa…f' with tanh / sigmoid / identity hidden activations, 2 to 6 linear layers (MAX_LAYERS),
+// the jet sets NS <= NF <= 4, every ansatz / residual program / sampler the thread kernel covers; hidden widths <= 64
+// (tests/test_gpu_tile.py) or <= 128 with at least one above 64 (tests/test_gpu_tile128.py).  Everything else
+// (residual layouts, sin/softplus/SiLU/GELU, wider layers, more layers, orders 3 / 4) stays on the thread kernels.
 #pragma once
 
 #include "pinn_step_kernel.cuh"
@@ -35,38 +40,55 @@
 namespace pinn {
 namespace wide {
 
-constexpr int T = 128;                 // points per tile
 constexpr int NT_MAX = 512;            // threads per CTA (template NT = 256 or 512): thread = (point, 1/NH of the hidden units)
-constexpr int KW = 64;                 // padded hidden width
 constexpr int MAX_LAYERS = 6;          // linear layers (hidden levels H <= 5, hidden->hidden layers <= 4)
-constexpr int LDS = KW + 4;            // row stride (floats) of the [row][64] operands: conflict-free fragment loads
-constexpr int LXB = T + 4;             // row stride of the small right-hand sides [16][128 p]
+constexpr int TILE_FLOATS = 8192;      // points per tile x padded width: the same for both width classes
 
-// ---- shared memory map (bytes) ---------------------------------------------------------------------------------
-constexpr int S_W = 0;                                  // layer weights as B operand [64 n][LDS]
-constexpr int S_A = S_W + KW * LDS * 4;                 // A operand [128 p][LDS]: jets (forward), delta (reverse)
-constexpr int S_GB = S_A + T * LDS * 4;                 // weight-gradient B operand: post-activation a_{h-1} [128 p][LDS]
-constexpr int S_D = S_GB + T * LDS * 4;                 // GEMM result [128 p][LDS]
-constexpr int S_X = S_D + T * LDS * 4;                  // exchange area between the threads of a point [24][128]
-constexpr int S_XB = S_X + 24 * T * 4;                  // small right-hand sides [16 rows][LXB]
-constexpr int S_WACC = S_XB + 16 * LXB * 4;             // weight gradients of the hidden->hidden layers [4][64 j][64 m]
-constexpr int S_SMALL1 = S_WACC + (MAX_LAYERS - 2) * KW * KW * 4;  // level 1: first-layer W / b gradients [64 k][16]
-constexpr int S_OUT = S_SMALL1 + KW * 16 * 4;           // output-layer weight gradient [64 k][8]
-constexpr int S_SMALLH = S_OUT + KW * 8 * 4;            // level h >= 2: bias gradient of layer h-1 [4][64 j][8]
-constexpr int S_MISC = S_SMALLH + (MAX_LAYERS - 2) * KW * 8 * 4;   // biases, first-layer weights, scalars
-constexpr int MISC_FLOATS = 1536;
-constexpr int SMEM_BYTES = S_MISC + MISC_FLOATS * 4;
-constexpr int ACC_FLOATS = (S_MISC - S_WACC) / 4;       // every accumulator, zeroed once per launch
-static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one CTA");
+__host__ __device__ constexpr int ilog2(int x) { return x <= 1 ? 0 : 1 + ilog2(x >> 1); }
 
-// misc area (float offsets)
-constexpr int M_BIAS = 0;                       // [MAX_LAYERS][64]
-constexpr int M_W0 = M_BIAS + MAX_LAYERS * 64;  // first layer [64][8]
-constexpr int M_WD = M_W0 + 64 * 8;             // first layer applied to the direction vectors [6][64]
-constexpr int M_WOUT = M_WD + PINN_MAX_DIRS * 64;   // output layer weights [64]
-constexpr int M_SCAL = M_WOUT + 64;                 // per warp: loss, sbar, bout, vbar[4]  (8 floats each)
-constexpr int M_END = M_SCAL + 8 * (NT_MAX / 32);
-static_assert(M_END <= MISC_FLOATS, "misc area");
+// The geometry of one width class KW (padded hidden width, 64 or 128).  The tile shrinks as the width grows,
+// T = 8192 / KW points, so that every [T][KW] operand, the slab block of a (level, channel) and the work-item count
+// of the data-gradient GEMM stay the same size; a thread still owns 16 hidden units at 512 threads.
+template <int KW_>
+struct Tile {
+    static constexpr int KW = KW_;
+    static constexpr int T = TILE_FLOATS / KW;             // points per tile: 128 (KW = 64) or 64 (KW = 128)
+    static constexpr int KSH = ilog2(KW), TSH = ilog2(T);
+    static constexpr int LDS = KW + 4;                     // row stride (floats) of the [row][KW] operands: conflict-free fragment loads
+    static constexpr int LXB = T + 4;                      // row stride of the small right-hand sides [16][T p]
+    // the weight gradients of the hidden->hidden layers [4][KW j][KW m]: in shared memory at KW = 64; at KW = 128
+    // (256 KB) in this CTA's area of the workspace
+    static constexpr int WACC_FLOATS = (MAX_LAYERS - 2) * KW * KW;
+    static constexpr bool WACC_SMEM = KW == 64;
+
+    // ---- shared memory map (bytes) -----------------------------------------------------------------------------
+    static constexpr int S_W = 0;                          // layer weights as B operand [KW n][LDS]
+    static constexpr int S_A = S_W + KW * LDS * 4;         // A operand [T p][LDS]: jets (forward), delta (reverse)
+    static constexpr int S_GB = S_A + T * LDS * 4;         // weight-gradient B operand: post-activation a_{h-1} [T p][LDS]
+    static constexpr int S_D = S_GB + T * LDS * 4;         // GEMM result [T p][LDS]
+    static constexpr int S_X = S_D + T * LDS * 4;          // exchange area between the threads of a point [24][T]
+    static constexpr int S_XB = S_X + 24 * T * 4;          // small right-hand sides [16 rows][LXB]
+    static constexpr int S_WACC = S_XB + 16 * LXB * 4;     // hidden->hidden weight gradients (KW = 64 only)
+    static constexpr int S_SMALL1 = S_WACC + (WACC_SMEM ? WACC_FLOATS * 4 : 0);  // level 1: first-layer W / b gradients [KW k][16]
+    static constexpr int S_OUT = S_SMALL1 + KW * 16 * 4;   // output-layer weight gradient [KW k][8]
+    static constexpr int S_SMALLH = S_OUT + KW * 8 * 4;    // level h >= 2: bias gradient of layer h-1 [4][KW j][8]
+    static constexpr int S_MISC = S_SMALLH + (MAX_LAYERS - 2) * KW * 8 * 4;   // biases, first-layer weights, scalars
+    static constexpr int MISC_FLOATS = 24 * KW;
+    static constexpr int SMEM_BYTES = S_MISC + MISC_FLOATS * 4;
+    static constexpr int ACC_FLOATS = (S_MISC - S_WACC) / 4;   // every shared-memory accumulator, zeroed once per launch
+
+    // misc area (float offsets)
+    static constexpr int M_BIAS = 0;                           // [MAX_LAYERS][KW]
+    static constexpr int M_W0 = M_BIAS + MAX_LAYERS * KW;      // first layer [KW][8]
+    static constexpr int M_WD = M_W0 + KW * 8;                 // first layer applied to the direction vectors [6][KW]
+    static constexpr int M_WOUT = M_WD + PINN_MAX_DIRS * KW;   // output layer weights [KW]
+    static constexpr int M_SCAL = M_WOUT + KW;                 // per warp: loss, sbar, bout, vbar[4]  (8 floats each)
+    static constexpr int M_END = M_SCAL + 8 * (NT_MAX / 32);
+
+    static_assert(KW == 64 || KW == 128, "width classes");
+    static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one CTA");
+    static_assert(M_END <= MISC_FLOATS, "misc area");
+};
 
 // Split x into a TF32 high part and a TF32 remainder (3xTF32 products).
 __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
@@ -94,22 +116,26 @@ __device__ __forceinline__ void mma3(float (&d)[4], const uint32_t (&ah)[4], con
 // The slab block of one (level, channel) is laid out [k / 4][point][k % 4]: the 16-byte loads of a warp's 32
 // points are contiguous (4 cache lines per request instead of 32 with one 256-byte row per point).
 // `blk` points at this thread's first float4 of the block; units k0 .. k0+7 are two float4, T*4 floats apart.
+template <int T>
 __device__ __forceinline__ void ld8(const float* __restrict__ blk, int k0, float (&v)[8]) {
     const float* q = blk + (size_t)(k0 >> 2) * (T * 4);
     const float4 a = *reinterpret_cast<const float4*>(q), b = *reinterpret_cast<const float4*>(q + T * 4);
     v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
 }
+template <int T>
 __device__ __forceinline__ void st8(float* __restrict__ blk, int k0, const float (&v)[8]) {
     float* q = blk + (size_t)(k0 >> 2) * (T * 4);
     *reinterpret_cast<float4*>(q) = make_float4(v[0], v[1], v[2], v[3]);
     *reinterpret_cast<float4*>(q + T * 4) = make_float4(v[4], v[5], v[6], v[7]);
 }
-// units k0..k0+7 of row p of a [128][LDS] shared-memory operand
+// units k0..k0+7 of row p of a [T][LDS] shared-memory operand
+template <int LDS>
 __device__ __forceinline__ void st_row8(uint8_t* base, int p, int k0, const float (&v)[8]) {
     float* q = reinterpret_cast<float*>(base) + p * LDS + k0;
     *reinterpret_cast<float4*>(q) = make_float4(v[0], v[1], v[2], v[3]);
     *reinterpret_cast<float4*>(q + 4) = make_float4(v[4], v[5], v[6], v[7]);
 }
+template <int LDS>
 __device__ __forceinline__ void ld_row8(const uint8_t* base, int p, int k0, float (&v)[8]) {
     const float* q = reinterpret_cast<const float*>(base) + p * LDS + k0;
     const float4 a = *reinterpret_cast<const float4*>(q), b = *reinterpret_cast<const float4*>(q + 4);
@@ -119,33 +145,39 @@ __device__ __forceinline__ void ld_row8(const uint8_t* base, int p, int k0, floa
 __host__ __device__ inline int rup(int x, int m) { return (x + m - 1) / m * m; }
 // Slab blocks per CTA: level 1 keeps only its activations (its first-order jets do not depend on the point, its
 // second-order jets vanish), levels 2..H keep all C channels; the adjoint of level h-1 overwrites the dead slot (h, c).
+// A block is T x KW floats, the same in both width classes.
 __host__ __device__ inline size_t spill_floats_per_cta(int n_layers, int C) {
     const int upper = n_layers - 2 > 0 ? n_layers - 2 : 0;
-    return (size_t)(1 + upper * C) * T * KW;
+    return (size_t)(1 + upper * C) * TILE_FLOATS;
 }
 
-// Stage one layer's weights as the B operand of a GEMM ([n][k], zero padded to 64 x 64).
+// Stage one layer's weights as the B operand of a GEMM ([n][k], zero padded to KW x KW).
 //   forward  (transpose = false): B[n = out unit j][k = in unit m] = W[j][m]
 //   backward (transpose = true) : B[n = in unit m][k = out unit j] = W[j][m]
+template <int KW>
 __device__ __forceinline__ void stage_layer(uint8_t* smem, const float* __restrict__ params, const DevLayer& L, bool transpose) {
-    float* w_s = reinterpret_cast<float*>(smem + S_W);
+    using G = Tile<KW>;
+    float* w_s = reinterpret_cast<float*>(smem + G::S_W);
     for (int i = threadIdx.x; i < KW * KW; i += blockDim.x) {
-        const int n = i >> 6, k = i & 63;
+        const int n = i >> G::KSH, k = i & (KW - 1);
         const int j = transpose ? k : n, m = transpose ? n : k;
-        w_s[n * LDS + k] = (j < L.n_out && m < L.n_in) ? __ldg(params + L.w_off + j * L.n_in + m) : 0.0f;
+        w_s[n * G::LDS + k] = (j < L.n_out && m < L.n_in) ? __ldg(params + L.w_off + j * L.n_in + m) : 0.0f;
     }
 }
 
 // Fragment coordinates of mma.m16n8k8: g = row group, t = thread in group.
-// Columns [0, np) of  D[128 x np] = A[128 x kp] . B[np x kp]^T  (A, D: [128][LDS], B: [64][LDS]).
-// Work items (16-row block, 32-column half) are dealt to the warps.
+// Columns [0, np) of  D[T x np] = A[T x kp] . B[np x kp]^T  (A, D: [T][LDS], B: [KW][LDS]).
+// Work items (16-row block, 32-column block: T/16 x KW/32 = 16 of them) are dealt to the warps.
+template <int KW>
 __device__ __forceinline__ void gemm_rows(const uint8_t* smem, int kp, int np, int warp, int n_warps) {
-    const float* A = reinterpret_cast<const float*>(smem + S_A);
-    const float* B = reinterpret_cast<const float*>(smem + S_W);
-    float* D = reinterpret_cast<float*>(const_cast<uint8_t*>(smem) + S_D);
+    using G = Tile<KW>;
+    constexpr int LDS = G::LDS, CB = KW / 32;
+    const float* A = reinterpret_cast<const float*>(smem + G::S_A);
+    const float* B = reinterpret_cast<const float*>(smem + G::S_W);
+    float* D = reinterpret_cast<float*>(const_cast<uint8_t*>(smem) + G::S_D);
     const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-    for (int item = warp; item < 16; item += n_warps) {
-        const int r0 = (item >> 1) * 16, c0 = (item & 1) * 32;
+    for (int item = warp; item < (G::T / 16) * CB; item += n_warps) {
+        const int r0 = (item >> ilog2(CB)) * 16, c0 = (item & (CB - 1)) * 32;
         if (c0 >= np) continue;
         float acc[4][4];
 #pragma unroll
@@ -180,14 +212,18 @@ __device__ __forceinline__ void gemm_rows(const uint8_t* smem, int kp, int np, i
         }
     }
 }
-// ACC[64 j x 64 m] (row stride 64) += GA^T . GB over the 128 points of the tile (GA = S_A, GB = S_GB, both
-// [128 p][LDS]); rows j < mrows and columns m < ncols.  Work items: 16 x 16 blocks.
+// ACC[KW j x KW m] (row stride KW) += GA^T . GB over the T points of the tile (GA = S_A, GB = S_GB, both
+// [T p][LDS]); rows j < mrows and columns m < ncols.  Work items: 16 x 16 blocks.  ACC is in shared memory
+// (KW = 64) or in the workspace (KW = 128); either way each block has one owning warp, which adds the tiles in order.
+template <int KW>
 __device__ __forceinline__ void gemm_wgrad(uint8_t* smem, float* acc_s, int mrows, int ncols, int warp, int n_warps) {
-    const float* GA = reinterpret_cast<const float*>(smem + S_A);
-    const float* GB = reinterpret_cast<const float*>(smem + S_GB);
+    using G = Tile<KW>;
+    constexpr int LDS = G::LDS, MB = KW / 16;
+    const float* GA = reinterpret_cast<const float*>(smem + G::S_A);
+    const float* GB = reinterpret_cast<const float*>(smem + G::S_GB);
     const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-    for (int item = warp; item < 16; item += n_warps) {
-        const int j0 = (item >> 2) * 16, m0 = (item & 3) * 16;
+    for (int item = warp; item < MB * MB; item += n_warps) {
+        const int j0 = (item >> ilog2(MB)) * 16, m0 = (item & (MB - 1)) * 16;
         if (j0 >= mrows || m0 >= ncols) continue;
         float acc[2][4];
 #pragma unroll
@@ -195,7 +231,7 @@ __device__ __forceinline__ void gemm_wgrad(uint8_t* smem, float* acc_s, int mrow
 #pragma unroll
             for (int i = 0; i < 4; ++i) acc[nt][i] = 0.0f;
 #pragma unroll 2
-        for (int p0 = 0; p0 < T; p0 += 8) {
+        for (int p0 = 0; p0 < G::T; p0 += 8) {
             const float* pa = GA + (p0 + t) * LDS + j0 + g;
             uint32_t ah[4], al[4];
             split_tf32(pa[0], ah[0], al[0]);
@@ -219,25 +255,28 @@ __device__ __forceinline__ void gemm_wgrad(uint8_t* smem, float* acc_s, int mrow
         }
     }
 }
-// ACC[64 j x n] (row stride n) += GA^T . XB^T over the tile (XB: [16 rows][LXB]), n = 8 or 16.  The work items
+// ACC[KW j x n] (row stride n) += GA^T . XB^T over the tile (XB: [16 rows][LXB]), n = 8 or 16.  The work items
 // (16 x 8 blocks) are dealt from the last warp down, so that they land beside the items of gemm_wgrad.
+template <int KW>
 __device__ __forceinline__ void gemm_small(uint8_t* smem, float* acc_s, int n, int warp, int n_warps) {
-    const float* GA = reinterpret_cast<const float*>(smem + S_A);
-    const float* XB = reinterpret_cast<const float*>(smem + S_XB);
+    using G = Tile<KW>;
+    constexpr int LDS = G::LDS, MB = KW / 16;
+    const float* GA = reinterpret_cast<const float*>(smem + G::S_A);
+    const float* XB = reinterpret_cast<const float*>(smem + G::S_XB);
     const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-    const int n_items = 4 * (n >> 3);
+    const int n_items = MB * (n >> 3);
     for (int item = n_warps - 1 - warp; item < n_items; item += n_warps) {
-        const int j0 = (item & 3) * 16, r0 = (item >> 2) * 8;
+        const int j0 = (item & (MB - 1)) * 16, r0 = (item >> ilog2(MB)) * 8;
         float acc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
 #pragma unroll 2
-        for (int p0 = 0; p0 < T; p0 += 8) {
+        for (int p0 = 0; p0 < G::T; p0 += 8) {
             const float* pa = GA + (p0 + t) * LDS + j0 + g;
             uint32_t ah[4], al[4];
             split_tf32(pa[0], ah[0], al[0]);
             split_tf32(pa[8], ah[1], al[1]);
             split_tf32(pa[4 * LDS], ah[2], al[2]);
             split_tf32(pa[4 * LDS + 8], ah[3], al[3]);
-            const float* pb = XB + (r0 + g) * LXB + p0 + t;
+            const float* pb = XB + (r0 + g) * G::LXB + p0 + t;
             uint32_t bh0, bl0, bh1, bl1;
             split_tf32(pb[0], bh0, bl0);
             split_tf32(pb[4], bh1, bl1);
@@ -250,39 +289,53 @@ __device__ __forceinline__ void gemm_small(uint8_t* smem, float* acc_s, int n, i
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-template <int NF, int NS, int NT>
-__global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
+// The body of the kernels below.  KW: the width class (hidden widths <= 64 or <= 128).  FWD: the forward-only form
+// (pinn_forward), with NF = NS = 0: forward sweep of the value channel, ansatz, u of every point to a.out; no slab, no
+// reverse sweep.
+template <int NF, int NS, int NT, int KW, bool FWD>
+__device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
+    using G = Tile<KW>;
+    constexpr int T = G::T, LDS = G::LDS, LXB = G::LXB;
     constexpr int C = 1 + NF + NS;
     constexpr int NH = NT / T;               // threads per point: each owns KW / NH hidden units
     constexpr int QN = KW / NH / 8;          // 8-unit chunks per thread
+    static_assert(NH * T == NT && QN * 8 * NH == KW, "threads per point");
+    static_assert(!FWD || (NF == 0 && NS == 0), "the forward-only form carries the value channel only");
     extern __shared__ __align__(16) uint8_t smem[];
-    float* misc = reinterpret_cast<float*>(smem + S_MISC);
+    float* misc = reinterpret_cast<float*>(smem + G::S_MISC);
 
-    const int tid = threadIdx.x, p = tid & 127, kh = tid >> 7, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, p = tid & (T - 1), kh = tid >> G::TSH, warp = tid >> 5, lane = tid & 31;
     const int warp_u = __shfl_sync(0xffffffffu, tid >> 5, 0);        // the same number, provably warp-uniform
     const int Ln = P.n_layers, H = Ln - 1;
     const int n_out_floats = P.n_params + 4;
+    // hidden->hidden weight-gradient accumulators [4][KW][KW]: shared memory, or this CTA's area of the workspace
+    float* const wacc_base = G::WACC_SMEM ? reinterpret_cast<float*>(smem + G::S_WACC)
+                                          : a.wacc + (size_t)blockIdx.x * G::WACC_FLOATS;
 
     pdl_wait();                                    // the previous step (its parameter update) is complete and visible
     pdl_launch_dependents();
     // ---- one-time setup: constants, zeroed accumulators -----------------------------------------------------------
-    for (int i = tid; i < MISC_FLOATS; i += NT) misc[i] = 0.0f;
-    for (int i = tid; i < 16 * LXB; i += NT) reinterpret_cast<float*>(smem + S_XB)[i] = 0.0f;
-    for (int i = tid; i < ACC_FLOATS; i += NT) reinterpret_cast<float*>(smem + S_WACC)[i] = 0.0f;
+    for (int i = tid; i < G::MISC_FLOATS; i += NT) misc[i] = 0.0f;
+    for (int i = tid; i < 16 * LXB; i += NT) reinterpret_cast<float*>(smem + G::S_XB)[i] = 0.0f;
+    for (int i = tid; i < G::ACC_FLOATS; i += NT) reinterpret_cast<float*>(smem + G::S_WACC)[i] = 0.0f;
+    if constexpr (!G::WACC_SMEM && !FWD) {
+        const int n4 = (Ln > 2 ? Ln - 2 : 0) * KW * KW / 4;          // the layers in use
+        for (int i = tid; i < n4; i += NT) reinterpret_cast<float4*>(wacc_base)[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    }
     __syncthreads();
     {
         // biases of every layer, first-layer weights and their products with the direction vectors, output weights
         for (int l = 0; l < Ln; ++l)
-            for (int j = tid; j < P.layer[l].n_out; j += NT) misc[M_BIAS + l * 64 + j] = __ldg(a.params + P.layer[l].b_off + j);
+            for (int j = tid; j < P.layer[l].n_out; j += NT) misc[G::M_BIAS + l * KW + j] = __ldg(a.params + P.layer[l].b_off + j);
         const DevLayer& L0 = P.layer[0];
-        for (int i = tid; i < L0.n_out * L0.n_in; i += NT) misc[M_W0 + (i / L0.n_in) * 8 + (i % L0.n_in)] = __ldg(a.params + L0.w_off + i);
-        for (int i = tid; i < NF * 64; i += NT) {
-            const int d = i >> 6, k = i & 63;
+        for (int i = tid; i < L0.n_out * L0.n_in; i += NT) misc[G::M_W0 + (i / L0.n_in) * 8 + (i % L0.n_in)] = __ldg(a.params + L0.w_off + i);
+        for (int i = tid; i < NF * KW; i += NT) {
+            const int d = i >> G::KSH, k = i & (KW - 1);
             float sum = 0.0f;
             if (k < L0.n_out) for (int q = 0; q < L0.n_in; ++q) sum = fmaf(__ldg(a.params + L0.w_off + k * L0.n_in + q), P.dir_vec[d][q], sum);
-            misc[M_WD + d * 64 + k] = sum;
+            misc[G::M_WD + d * KW + k] = sum;
         }
-        for (int k = tid; k < P.layer[H].n_in; k += NT) misc[M_WOUT + k] = __ldg(a.params + P.layer[H].w_off + k);
+        for (int k = tid; k < P.layer[H].n_in; k += NT) misc[G::M_WOUT + k] = __ldg(a.params + P.layer[H].w_off + k);
     }
     __syncthreads();
 
@@ -292,9 +345,9 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
         const int b = (h == 1) ? 0 : 1 + (h - 2) * C + c;    // level 1 keeps channel 0 only
         return slab + (size_t)b * (T * KW) + p * 4;
     };
-    float* Xbuf = reinterpret_cast<float*>(smem + S_X);      // exchange area between the threads of a point
-    float* xb = reinterpret_cast<float*>(smem + S_XB);       // small right-hand sides [16][LXB]
-    float* st = reinterpret_cast<float*>(smem + S_A) + p;    // ansatz / program scratch rows (stride T), A/GB area
+    float* Xbuf = reinterpret_cast<float*>(smem + G::S_X);      // exchange area between the threads of a point
+    float* xb = reinterpret_cast<float*>(smem + G::S_XB);       // small right-hand sides [16][LXB]
+    float* st = reinterpret_cast<float*>(smem + G::S_A) + p;    // ansatz / program scratch rows (stride T), A/GB area
     constexpr int RS = T;
     const int kbeg = kh * (KW / NH);
 
@@ -316,9 +369,9 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
     auto ldz = [&](int h, int c, int k0, float (&v)[8]) {
         if (h == 1) {
 #pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = (c <= NF) ? misc[M_WD + (c - 1) * 64 + k0 + i] : 0.0f;
+            for (int i = 0; i < 8; ++i) v[i] = (c <= NF) ? misc[G::M_WD + (c - 1) * KW + k0 + i] : 0.0f;
         } else {
-            ld8(row(h, c), k0, v);
+            ld8<T>(row(h, c), k0, v);
         }
     };
     // A jet set is walked in GROUPS: group 0 = the value channel; group 1+d = direction d, i.e. its first-order
@@ -349,7 +402,7 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
             }
         }
     };
-    auto put_A = [&](int k0, const float (&v)[8]) { st_row8(smem + S_A, p, k0, v); };   // A operand of the next GEMM
+    auto put_A = [&](int k0, const float (&v)[8]) { st_row8<LDS>(smem + G::S_A, p, k0, v); };   // A operand of the next GEMM
 
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const long long pl = tile * T + p;
@@ -386,12 +439,12 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
                 const int k0 = kbeg + q * 8;
 #pragma unroll
                 for (int i = 0; i < 8; ++i) {
-                    float z = misc[M_BIAS + k0 + i];
+                    float z = misc[G::M_BIAS + k0 + i];
 #pragma unroll
-                    for (int j = 0; j < PINN_MAX_DIMS; ++j) z = fmaf(misc[M_W0 + (k0 + i) * 8 + j], x[j], z);
+                    for (int j = 0; j < PINN_MAX_DIMS; ++j) z = fmaf(misc[G::M_W0 + (k0 + i) * 8 + j], x[j], z);
                     a0h[q][i] = act_store<false>(kc, z);
                 }
-                st8(row(1, 0), k0, a0h[q]);
+                if constexpr (!FWD) st8<T>(row(1, 0), k0, a0h[q]);
             }
         }
         // levels 2..H and the output: one GEMM per channel
@@ -402,7 +455,7 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
             const ActC kc = make_actc(P.layer[h - 1].act);
             const ActC kn = make_actc(L.act);
             __syncthreads();                                 // nobody reads the previous W any more
-            stage_layer(smem, a.params, L, false);
+            stage_layer<KW>(smem, a.params, L, false);
             float a0n[QN][8];                                // activations of level h+1 as they come out of channel 0
             auto finish = [&](int c) {                       // accumulator -> level h+1 (or the network output)
                 if (h < H) {
@@ -410,22 +463,22 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
                     for (int q = 0; q < QN; ++q) {
                         const int n0 = kbeg + q * 8;
                         float z[8];
-                        if (n0 < np) ld_row8(smem + S_D, p, n0, z);
+                        if (n0 < np) ld_row8<LDS>(smem + G::S_D, p, n0, z);
                         else {
 #pragma unroll
                             for (int i = 0; i < 8; ++i) z[i] = 0.0f;
                         }
                         if (c == 0) {
 #pragma unroll
-                            for (int i = 0; i < 8; ++i) { z[i] = act_store<false>(kn, z[i] + misc[M_BIAS + h * 64 + n0 + i]); a0n[q][i] = z[i]; }
+                            for (int i = 0; i < 8; ++i) { z[i] = act_store<false>(kn, z[i] + misc[G::M_BIAS + h * KW + n0 + i]); a0n[q][i] = z[i]; }
                         }
-                        st8(row(h + 1, c), n0, z);
+                        if constexpr (!FWD) st8<T>(row(h + 1, c), n0, z);
                     }
                 } else {
-                    N[c] = reinterpret_cast<const float*>(smem + S_D)[p * LDS] + (c == 0 ? misc[M_BIAS + H * 64] : 0.0f);
+                    N[c] = reinterpret_cast<const float*>(smem + G::S_D)[p * LDS] + (c == 0 ? misc[G::M_BIAS + H * KW] : 0.0f);
                 }
             };
-            auto gemm = [&](int w) { gemm_rows(smem, kp, np, w, NT / 32); };
+            auto gemm = [&](int w) { gemm_rows<KW>(smem, kp, np, w, NT / 32); };
             for (int g = 0; g <= NF; ++g) {
                 const int cy = group_y(g);
                 float stash[QN][8];
@@ -474,36 +527,41 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
             AnsatzState<NF, NS> as;
             float u[C];
             ansatz_forward<NF, NS, true>(P, coords, RS, log_scale, N, icj, as, u);
+            if constexpr (FWD) {
+                if (valid) a.out[pl] = u[0];
+            } else {
 #pragma unroll
-            for (int c = 0; c < C; ++c) scr[(size_t)c * RS] = u[c];
-            eval_prog(P.eq, P.n_eq, scr, RS, coords, a.params, P.var_off);
-            const float r = scr[(size_t)P.eq_out[0] * RS];
-            const float rb = valid ? 2.0f * r * a.inv_n : 0.0f;
-            if (valid) acc_loss = fmaf(r * a.inv_n, r, acc_loss);
-            if (a.residual && valid) a.residual[pl] = r;
-            float ub[C];
+                for (int c = 0; c < C; ++c) scr[(size_t)c * RS] = u[c];
+                eval_prog(P.eq, P.n_eq, scr, RS, coords, a.params, P.var_off);
+                const float r = scr[(size_t)P.eq_out[0] * RS];
+                const float rb = valid ? 2.0f * r * a.inv_n : 0.0f;
+                if (valid) acc_loss = fmaf(r * a.inv_n, r, acc_loss);
+                if (a.residual && valid) a.residual[pl] = r;
+                float ub[C];
 #pragma unroll
-            for (int c = 0; c < C; ++c) ub[c] = rb * scr[(size_t)P.eq_out[1 + c] * RS];
+                for (int c = 0; c < C; ++c) ub[c] = rb * scr[(size_t)P.eq_out[1 + c] * RS];
 #pragma unroll
-            for (int i = 0; i < PINN_MAX_VARS; ++i)
-                if (i < P.n_vars) acc_vbar[i] = fmaf(rb, scr[(size_t)P.eq_out[1 + C + i] * RS], acc_vbar[i]);
-            if (P.ic_has_vars) {
+                for (int i = 0; i < PINN_MAX_VARS; ++i)
+                    if (i < P.n_vars) acc_vbar[i] = fmaf(rb, scr[(size_t)P.eq_out[1 + C + i] * RS], acc_vbar[i]);
+                if (P.ic_has_vars) {
 #pragma unroll
-                for (int i = 0; i < PINN_MAX_VARS; ++i) {
-                    if (i < P.n_vars) {
+                    for (int i = 0; i < PINN_MAX_VARS; ++i) {
+                        if (i < P.n_vars) {
 #pragma unroll
-                        for (int c = 0; c < C; ++c)
-                            acc_vbar[i] = fmaf(ub[c], scr[(size_t)P.ic_out[C * (1 + i) + c] * RS], acc_vbar[i]);
+                            for (int c = 0; c < C; ++c)
+                                acc_vbar[i] = fmaf(ub[c], scr[(size_t)P.ic_out[C * (1 + i) + c] * RS], acc_vbar[i]);
+                        }
                     }
                 }
-            }
-            acc_sbar += ansatz_adjoint<NF, NS>(P, as, ub, Nb);
-            acc_bout += Nb[0];
-            // the adjoint seed of the point goes to the exchange area (rows 0..C-1): every thread of the point reads
-            // it from there when it needs it, instead of carrying C registers through the reverse sweep
+                acc_sbar += ansatz_adjoint<NF, NS>(P, as, ub, Nb);
+                acc_bout += Nb[0];
+                // the adjoint seed of the point goes to the exchange area (rows 0..C-1): every thread of the point reads
+                // it from there when it needs it, instead of carrying C registers through the reverse sweep
 #pragma unroll
-            for (int c = 0; c < C; ++c) Xbuf[c * T + p] = Nb[c];
+                for (int c = 0; c < C; ++c) Xbuf[c * T + p] = Nb[c];
+            }
         }
+        if constexpr (FWD) continue;                         // the forward-only form ends its tile here
         auto nb_of = [&](int c) { return Xbuf[c * T + p]; };
         __syncthreads();
 
@@ -535,7 +593,7 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
                 put_A(k0, t);
             }
             if (kh == 0) xb[p] = 1.0f;
-            sync_issue([&](int w) { gemm_small(smem, reinterpret_cast<float*>(smem + S_OUT), 8, w, NT / 32); });
+            sync_issue([&](int w) { gemm_small<KW>(smem, reinterpret_cast<float*>(smem + G::S_OUT), 8, w, NT / 32); });
         }
         // rounds H..1: adjoint through the activation of level h, then (h >= 2) through the linear layer below it
         for (int h = H; h >= 1; --h) {
@@ -545,11 +603,11 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
             const int kp = rup(L.n_out, 8), np = rup(L.n_in, 16);
             if (h >= 2) {
                 __syncthreads();
-                stage_layer(smem, a.params, L, true);
+                stage_layer<KW>(smem, a.params, L, true);
             }
             if (h < H) {                                     // (at the top level the forward sweep left them in registers)
 #pragma unroll
-                for (int q = 0; q < QN; ++q) ld8(row(h, 0), kbeg + q * 8, a0h[q]);
+                for (int q = 0; q < QN; ++q) ld8<T>(row(h, 0), kbeg + q * 8, a0h[q]);
             }
             float R[QN][8];                                  // running sum of the value-channel adjoint
 #pragma unroll
@@ -561,9 +619,9 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
                 if (h == H) {
                     const float nb = nb_of(c);
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) v[i] = misc[M_WOUT + k0 + i] * nb;
+                    for (int i = 0; i < 8; ++i) v[i] = misc[G::M_WOUT + k0 + i] * nb;
                 } else {
-                    ld8(row(h + 1, c), k0, v);
+                    ld8<T>(row(h + 1, c), k0, v);
                 }
             };
             // operands of channel c are in place (A = GA = delta, and for h >= 2 GB = a_{h-1,c})
@@ -582,29 +640,29 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
                     // weight gradient (16 x 16 blocks) and, on the value channel, the bias gradient (dealt from the
                     // last warp down)
                     sync_issue([&](int w) {
-                        gemm_rows(smem, kp, np, w, NT / 32);
-                        gemm_wgrad(smem, reinterpret_cast<float*>(smem + S_WACC) + (h - 2) * KW * KW, L.n_out, L.n_in, w, NT / 32);
-                        if (c == 0) gemm_small(smem, reinterpret_cast<float*>(smem + S_SMALLH) + (h - 2) * KW * 8, 8, w, NT / 32);
+                        gemm_rows<KW>(smem, kp, np, w, NT / 32);
+                        gemm_wgrad<KW>(smem, wacc_base + (h - 2) * KW * KW, L.n_out, L.n_in, w, NT / 32);
+                        if (c == 0) gemm_small<KW>(smem, reinterpret_cast<float*>(smem + G::S_SMALLH) + (h - 2) * KW * 8, 8, w, NT / 32);
                     });
                     float* dst = row(h, c);                  // abar_{h-1,c} takes the dead slot of (h, c)
 #pragma unroll
                     for (int q = 0; q < QN; ++q) {
                         const int n0 = kbeg + q * 8;
                         float z[8];
-                        if (n0 < np) ld_row8(smem + S_D, p, n0, z);
+                        if (n0 < np) ld_row8<LDS>(smem + G::S_D, p, n0, z);
                         else {
 #pragma unroll
                             for (int i = 0; i < 8; ++i) z[i] = 0.0f;
                         }
-                        st8(dst, n0, z);
+                        st8<T>(dst, n0, z);
                     }
                 } else {                                     // level 1: only the first layer's own gradients
-                    sync_issue([&](int w) { gemm_small(smem, reinterpret_cast<float*>(smem + S_SMALL1), 16, w, NT / 32); });
+                    sync_issue([&](int w) { gemm_small<KW>(smem, reinterpret_cast<float*>(smem + G::S_SMALL1), 16, w, NT / 32); });
                 }
             };
             auto put_ops = [&](int k0, const float (&delta)[8], const float (&below)[8]) {
                 put_A(k0, delta);                            // A of the data gradient and GA of the reductions
-                if (h >= 2) st_row8(smem + S_GB, p, k0, below);
+                if (h >= 2) st_row8<LDS>(smem + G::S_GB, p, k0, below);
             };
             // directions first (pairs: second-order channel, then its first-order partner), the value channel last
             for (int gg = 1; gg <= NF + 1; ++gg) {
@@ -618,7 +676,7 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
                     const float (&a0)[8] = a0h[q];
                     if (h >= 2) {
                         float a0l[8];
-                        ld8(row(h - 1, 0), k0, a0l);
+                        ld8<T>(row(h - 1, 0), k0, a0l);
                         post_group(h - 1, g, k0, kb, a0l, bx, by);
                     }
                     if (g == 0) {
@@ -673,12 +731,14 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
         }
     }
 
+    if constexpr (FWD) return;
+
     // ---- read the accumulators out: this CTA's partial [grads | loss] ------------------------------------------------
     float* mine = a.partials + (size_t)blockIdx.x * n_out_floats;
     for (int i = tid; i < n_out_floats; i += NT) mine[i] = 0.0f;
     {
         // per-warp slots, summed in warp order below: no float atomics, bit-reproducible run to run
-        float* slot = misc + M_SCAL + 8 * warp;
+        float* slot = misc + G::M_SCAL + 8 * warp;
         float v = warp_sum(acc_loss);
         if (lane == 0) slot[0] = v;
         v = warp_sum(acc_sbar);
@@ -693,21 +753,21 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
     }
     __syncthreads();
     {
-        const float* wacc = reinterpret_cast<const float*>(smem + S_WACC);
-        const float* smallh = reinterpret_cast<const float*>(smem + S_SMALLH);
+        const float* wacc = wacc_base;
+        const float* smallh = reinterpret_cast<const float*>(smem + G::S_SMALLH);
         for (int li = 0; li + 2 < Ln; ++li) {               // hidden->hidden layer li+1
             const DevLayer& L = P.layer[li + 1];
             for (int i = tid; i < L.n_out * L.n_in; i += NT)
                 mine[L.w_off + i] = wacc[li * KW * KW + (i / L.n_in) * KW + i % L.n_in];
             for (int j = tid; j < L.n_out; j += NT) mine[L.b_off + j] = smallh[li * KW * 8 + j * 8];   // bias gradient
         }
-        const float* small1 = reinterpret_cast<const float*>(smem + S_SMALL1);   // [j][0] bias, [j][1 + i] weights
+        const float* small1 = reinterpret_cast<const float*>(smem + G::S_SMALL1);   // [j][0] bias, [j][1 + i] weights
         const DevLayer& L0 = P.layer[0];
         for (int j = tid; j < L0.n_out; j += NT) {
             mine[L0.b_off + j] = small1[j * 16];
             for (int i = 0; i < L0.n_in; ++i) mine[L0.w_off + j * L0.n_in + i] = small1[j * 16 + 1 + i];
         }
-        const float* outw = reinterpret_cast<const float*>(smem + S_OUT);
+        const float* outw = reinterpret_cast<const float*>(smem + G::S_OUT);
         const DevLayer& LO = P.layer[H];
         for (int j = tid; j < LO.n_in; j += NT) mine[LO.w_off + j] = outw[j * 8];
     }
@@ -716,7 +776,7 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
 #pragma unroll
         for (int i = 0; i < 3 + PINN_MAX_VARS; ++i) {
             float t = 0.0f;
-            for (int w = 0; w < NT / 32; ++w) t += misc[M_SCAL + 8 * w + i];
+            for (int w = 0; w < NT / 32; ++w) t += misc[G::M_SCAL + 8 * w + i];
             sc[i] = t;
         }
         mine[P.n_params] = sc[0];
@@ -727,6 +787,19 @@ __global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant_
     __syncthreads();
     finish_grid(a, n_out_floats);
 }
+
+// hidden widths <= 64: 128-point tiles, NT = 512 (four threads per point) or 256 (two)
+template <int NF, int NS, int NT>
+__global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
+    wide_step<NF, NS, NT, 64, false>(P, a);
+}
+// hidden widths <= 128: 64-point tiles, eight threads per point
+template <int NF, int NS>
+__global__ void __launch_bounds__(512, 1) wide128_step_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
+    wide_step<NF, NS, 512, 128, false>(P, a);
+}
+// pinn_forward of the networks only the 128-wide class holds: u of every point to a.out
+__global__ void __launch_bounds__(512, 1) wide128_forward_kernel(const __grid_constant__ DevPlan P, const StepArgs a);
 
 }  // namespace wide
 }  // namespace pinn

@@ -39,6 +39,9 @@ def main():
         solver.fit(niters=30, batch_size=100001, lr=0.005)          # odd size: uneven shards
     else:                                  # a registry problem, e.g. wave3d: the tensor-core tile kernel under data parallelism
         import problems as P
+        import problems_wide as PW         # ... or a 128-wide network (poisson_wide128)
+        if problem in PW.PROBLEMS:
+            P = PW
         cfg = P.PROBLEMS[problem]
         solver = Solver(P.bind(problem, D, lambda n, init: V(n, data=torch.Tensor([init]))), ndims=cfg['ndims'],
                         nparams=cfg['nparams'], initial_condition=cfg['ic'], boundary_condition=cfg['bc'],
