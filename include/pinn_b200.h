@@ -123,7 +123,8 @@ typedef struct PinnColumn {
  * Everything that defines one `Solver`: network, ansatz, derivative jet set, residual.
  *
  * Network (reference ConvBlockModel.forward model_torch.py:170-172, layouts 'fa…f'):
- *   n_layers linear layers, widths[0] = ndims + nparams, widths[n_layers] = 1;
+ *   n_layers linear layers, widths[0] = ndims + nparams, widths[n_layers] = k, the number of outputs: 1, or 2..4 for
+ *   coupled systems (thread kernel, derivative order <= 2, nf <= 4; see Programs);
  *   act[l] is the activation applied AFTER linear layer l (0-based); act[n_layers-1] must
  *   be PINN_ACT_NONE.  skip_src[l] = s >= 0 adds the output of layer s (after ITS activation and skip)
  *   to the activated output of layer l (residual connections 'R … +').
@@ -152,6 +153,10 @@ typedef struct PinnColumn {
  *   assembled; ic_out[c] is the slot holding channel c of the jet of ic.  When the initial condition
  *   uses variables (ic_has_vars; e.g. README.md:112-118 `V('init', ...)`), ic_out[C*(1+i) + c] is the
  *   slot of d(ic jet channel c)/dV_i and those slots lie above every slot eq_prog writes.
+ *   Networks of k = 2..4 outputs: slots j*C + c are preloaded with channel c of component j; eq_out[0] is still the
+ *   residual; the partials dr/d(channel c of component j) form one contiguous block, slot eq_out[1] + j*C + c, so that
+ *   eq_out[1 + c] = eq_out[1] + c; eq_out[1 + C + i] is still dr/dV_i.  ic_out is unchanged (one initial condition,
+ *   shared by every component like the boundary value, boundary factor and time gate).
  */
 typedef struct PinnSpec {
     int32_t  abi_version;
@@ -368,7 +373,7 @@ int pinn_multi_step(const PinnPlan* plan, float* params, float* exp_avg, float* 
 
 /* Forward only: u = ansatz(net(x)) for explicit points — the work of Solver.predict
  * (model_torch.py:466-487) and of the `_forward` closure handed to constraints (:451-454).
- * u_out [n_points]. */
+ * u_out [n_points] for a network of one output, [n_points, k] row-major for k outputs. */
 int pinn_forward(const PinnPlan* plan,
                  const float* params,
                  const float* points,

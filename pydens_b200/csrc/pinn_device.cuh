@@ -1105,7 +1105,26 @@ PINN_HD void wgrad_input_layer(const DevLayer& L, const float* __restrict__ out_
 template <int NF, int NS>
 struct PointPartials { float loss, sbar, vbar[PINN_MAX_VARS]; };
 
-template <int NF, int NS, int JF, bool GEN = true>
+// u_c = S v_c + ic_c: the variables of the initial condition pick up sum_c ub_c d(ic jet channel c)/dV_i.
+template <int NF, int NS>
+PINN_HD void ic_var_partials(const DevPlan& P, const float* __restrict__ scr, int RS, const float (&ub)[1 + NF + NS],
+                             PointPartials<NF, NS>& part) {
+    constexpr int C = 1 + NF + NS;
+#pragma unroll
+    for (int i = 0; i < PINN_MAX_VARS; ++i) {
+        if (i < P.n_vars) {
+#pragma unroll
+            for (int c = 0; c < C; ++c)
+                part.vbar[i] = fmaf(ub[c], scr[(size_t)P.ic_out[C * (1 + i) + c] * RS], part.vbar[i]);
+        }
+    }
+}
+
+// MULTI: a network of k = P.layer[n_layers-1].n_out in 2..4 outputs (coupled systems).  The k output jets live in the
+// output layer's storage rows (unit j, channel c), never in registers; the ansatz is applied to every component with
+// the shared boundary factor and time gate; the residual program finds channel c of component j in slot j*C + c and
+// leaves dr/d(that channel) in slot eq_out[1] + j*C + c.
+template <int NF, int NS, int JF, bool GEN = true, bool MULTI = false>
 PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weights */,
                          const float* __restrict__ pvals /* flat params (for log_scale, V) */,
                          float* __restrict__ st, int RS, bool valid, float inv_n,
@@ -1116,9 +1135,9 @@ PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weigh
     float* units = st + (size_t)P.row_units * RS;
     float* scr = st + (size_t)P.row_scr * RS;
 
-    // ---- forward through the hidden layers ----
+    // ---- forward through the hidden layers (and, for k outputs, the output layer: its k jets go to storage) ----
 #pragma unroll 1
-    for (int l = 0; l + 1 < Ln; ++l) {
+    for (int l = 0; l + (MULTI ? 0 : 1) < Ln; ++l) {
         const DevLayer& L = P.layer[l];
         int in_act = PINN_ACT_NONE;
         const float* in_rows = (l == 0) ? coords : layer_output<GEN>(P, l - 1, units, C, RS, in_act);
@@ -1127,7 +1146,7 @@ PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weigh
         if (GEN && L.skip_src >= 0) skip_sum_pass<NF, NS>(P, l, units, RS);
     }
     float N[C];
-    {
+    if constexpr (!MULTI) {
         const DevLayer& L = P.layer[Ln - 1];
         int in_act = PINN_ACT_NONE;
         const float* in_rows = (Ln == 1) ? coords : layer_output<GEN>(P, Ln - 2, units, C, RS, in_act);
@@ -1146,39 +1165,60 @@ PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weigh
     float log_scale = pvals[P.log_scale_off];
     AnsatzState<NF, NS> as;
     float u[C];
-    ansatz_forward<NF, NS, GEN>(P, coords, RS, log_scale, N, icj, as, u);
+    float* top_rows = units + (size_t)P.layer[Ln - 1].unit_base * C * RS;
+    const int n_out = MULTI ? P.layer[Ln - 1].n_out : 1;
+    if constexpr (MULTI) {
+#pragma unroll 1
+        for (int j = 0; j < n_out; ++j) {
 #pragma unroll
-    for (int c = 0; c < C; ++c) scr[(size_t)c * RS] = u[c];
+            for (int c = 0; c < C; ++c) N[c] = top_rows[((size_t)j * C + c) * RS];
+            ansatz_forward<NF, NS, GEN>(P, coords, RS, log_scale, N, icj, as, u);
+#pragma unroll
+            for (int c = 0; c < C; ++c) scr[((size_t)j * C + c) * RS] = u[c];
+        }
+    } else {
+        ansatz_forward<NF, NS, GEN>(P, coords, RS, log_scale, N, icj, as, u);
+#pragma unroll
+        for (int c = 0; c < C; ++c) scr[(size_t)c * RS] = u[c];
+    }
     eval_prog(P.eq, P.n_eq, scr, RS, coords, pvals, P.var_off);
     float r = scr[(size_t)P.eq_out[0] * RS];
     float rb = valid ? 2.0f * r * inv_n : 0.0f;
     if (valid) part.loss = fmaf(r * inv_n, r, part.loss);
-    float ub[C];
+    if constexpr (MULTI) {
 #pragma unroll
-    for (int c = 0; c < C; ++c) ub[c] = rb * scr[(size_t)P.eq_out[1 + c] * RS];
+        for (int i = 0; i < PINN_MAX_VARS; ++i)
+            if (i < P.n_vars) part.vbar[i] = fmaf(rb, scr[(size_t)P.eq_out[1 + C + i] * RS], part.vbar[i]);
+        // adjoint of the ansatz, one component at a time: the seeds come from the block of partials
+#pragma unroll 1
+        for (int j = 0; j < n_out; ++j) {
+            float ub[C];
 #pragma unroll
-    for (int i = 0; i < PINN_MAX_VARS; ++i)
-        if (i < P.n_vars) part.vbar[i] = fmaf(rb, scr[(size_t)P.eq_out[1 + C + i] * RS], part.vbar[i]);
-    if (GEN && P.ic_has_vars) {                // u_c = S v_c + ic_c: variables of the initial condition
+            for (int c = 0; c < C; ++c) ub[c] = rb * scr[(size_t)(P.eq_out[1] + j * C + c) * RS];
+            if (P.ic_has_vars) ic_var_partials<NF, NS>(P, scr, RS, ub, part);
 #pragma unroll
-        for (int i = 0; i < PINN_MAX_VARS; ++i) {
-            if (i < P.n_vars) {
+            for (int c = 0; c < C; ++c) N[c] = top_rows[((size_t)j * C + c) * RS];
+            ansatz_forward<NF, NS, GEN>(P, coords, RS, log_scale, N, icj, as, u);     // component j's ansatz state again
+            float Nb[C];
+            part.sbar += ansatz_adjoint<NF, NS>(P, as, ub, Nb);
 #pragma unroll
-                for (int c = 0; c < C; ++c)
-                    part.vbar[i] = fmaf(ub[c], scr[(size_t)P.ic_out[C * (1 + i) + c] * RS], part.vbar[i]);
-            }
+            for (int c = 0; c < C; ++c) top_rows[((size_t)j * C + c) * RS] = Nb[c];   // the reverse sweep starts here
         }
-    }
-
-    float Nb[C];
-    part.sbar += ansatz_adjoint<NF, NS>(P, as, ub, Nb);
-
-    // ---- reverse sweep ----
-    {
-        const DevLayer& L = P.layer[Ln - 1];
-        float* out_rows = units + (size_t)L.unit_base * C * RS;
+    } else {
+        float ub[C];
 #pragma unroll
-        for (int c = 0; c < C; ++c) out_rows[(size_t)c * RS] = Nb[c];
+        for (int c = 0; c < C; ++c) ub[c] = rb * scr[(size_t)P.eq_out[1 + c] * RS];
+#pragma unroll
+        for (int i = 0; i < PINN_MAX_VARS; ++i)
+            if (i < P.n_vars) part.vbar[i] = fmaf(rb, scr[(size_t)P.eq_out[1 + C + i] * RS], part.vbar[i]);
+        if (GEN && P.ic_has_vars) ic_var_partials<NF, NS>(P, scr, RS, ub, part);
+
+        float Nb[C];
+        part.sbar += ansatz_adjoint<NF, NS>(P, as, ub, Nb);
+
+        // ---- reverse sweep ----
+#pragma unroll
+        for (int c = 0; c < C; ++c) top_rows[(size_t)c * RS] = Nb[c];
     }
 #pragma unroll 1
     for (int l = Ln - 1; l >= 1; --l) {
@@ -1207,7 +1247,8 @@ PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weigh
 }
 
 // Forward-only value u(x) for one point (predict path): no jets (NF = NS = 0).
-template <int JF>
+// MULTI (k = P.layer[n_layers-1].n_out outputs): component j of u is left in scratch row j, and component 0 returned.
+template <int JF, bool MULTI = false>
 PINN_HD float point_forward(const DevPlan& P, const float* __restrict__ sw, const float* __restrict__ pvals,
                             float* __restrict__ st, int RS, int row_scr_fwd) {
     const int Ln = P.n_layers;
@@ -1215,7 +1256,7 @@ PINN_HD float point_forward(const DevPlan& P, const float* __restrict__ sw, cons
     float* units = st + (size_t)P.row_units * RS;
     float* scr = st + (size_t)row_scr_fwd * RS;
     float dummy_dir[1] = {0.0f};
-    for (int l = 0; l + 1 < Ln; ++l) {
+    for (int l = 0; l + (MULTI ? 0 : 1) < Ln; ++l) {
         const DevLayer& L = P.layer[l];
         int in_act = PINN_ACT_NONE;
         const float* in_rows = (l == 0) ? coords : layer_output(P, l - 1, units, 1, RS, in_act);
@@ -1223,7 +1264,7 @@ PINN_HD float point_forward(const DevPlan& P, const float* __restrict__ sw, cons
         if (L.skip_src >= 0) skip_sum_pass<0, 0>(P, l, units, RS);
     }
     float N[1];
-    {
+    if constexpr (!MULTI) {
         const DevLayer& L = P.layer[Ln - 1];
         int in_act = PINN_ACT_NONE;
         const float* in_rows = (Ln == 1) ? coords : layer_output(P, Ln - 2, units, 1, RS, in_act);
@@ -1236,8 +1277,20 @@ PINN_HD float point_forward(const DevPlan& P, const float* __restrict__ sw, cons
     }
     AnsatzState<0, 0> as;
     float u[1];
-    ansatz_forward<0, 0>(P, coords, RS, pvals[P.log_scale_off], N, icj, as, u);
-    return u[0];
+    if constexpr (MULTI) {
+        const float* top_rows = units + (size_t)P.layer[Ln - 1].unit_base * RS;
+        float u0 = 0.0f;
+        for (int j = 0; j < P.layer[Ln - 1].n_out; ++j) {
+            N[0] = top_rows[(size_t)j * RS];
+            ansatz_forward<0, 0>(P, coords, RS, pvals[P.log_scale_off], N, icj, as, u);
+            scr[(size_t)j * RS] = u[0];
+            if (j == 0) u0 = u[0];
+        }
+        return u0;
+    } else {
+        ansatz_forward<0, 0>(P, coords, RS, pvals[P.log_scale_off], N, icj, as, u);
+        return u[0];
+    }
 }
 
 }  // namespace pinn

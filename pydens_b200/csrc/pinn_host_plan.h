@@ -40,8 +40,10 @@ inline int validate_prog(const PinnInstr* prog, int n, int n_slots, int total, i
 inline int spec_order(const PinnSpec* s) { return s->order >= 3 ? s->order : 2; }
 inline int spec_channels(const PinnSpec* s) { return s->order >= 3 ? 1 + s->nf * s->order : 1 + s->nf + s->ns; }
 
-// Fills `h` (device plan, minus anything that needs a device) and the forward-only row layout.
-inline int build_dev_plan(const PinnSpec* s, DevPlan& h, int& fwd_rows, int& fwd_row_scr, char* msg, size_t msg_len) {
+// Fills `h` (device plan, minus anything that needs a device) and the forward-only row layout.  `max_out`: the most
+// network outputs the caller's kernels take — 1 for the one-output code, 4 where the coupled form runs too.
+inline int build_dev_plan(const PinnSpec* s, DevPlan& h, int& fwd_rows, int& fwd_row_scr, char* msg, size_t msg_len,
+                          int max_out = 1) {
     if (s->abi_version != PINN_ABI_VERSION)
         PINN_PLAN_FAIL(PINN_E_INVALID, "spec abi_version %d != library %d", s->abi_version, PINN_ABI_VERSION);
     const int Ln = s->n_layers;
@@ -49,7 +51,8 @@ inline int build_dev_plan(const PinnSpec* s, DevPlan& h, int& fwd_rows, int& fwd
     const int total = s->ndims + s->nparams;
     if (s->ndims < 1 || s->nparams < 0 || total > PINN_MAX_DIMS) PINN_PLAN_FAIL(PINN_E_INVALID, "ndims/nparams");
     if (s->widths[0] != total) PINN_PLAN_FAIL(PINN_E_INVALID, "widths[0]=%d != ndims+nparams=%d", s->widths[0], total);
-    if (s->widths[Ln] != 1) PINN_PLAN_FAIL(PINN_E_UNSUPPORTED, "output width %d (must be 1)", s->widths[Ln]);
+    const int n_out = s->widths[Ln];
+    if (n_out < 1 || n_out > max_out) PINN_PLAN_FAIL(PINN_E_UNSUPPORTED, "output width %d (1..%d)", n_out, max_out);
     if (s->act[Ln - 1] != PINN_ACT_NONE) PINN_PLAN_FAIL(PINN_E_UNSUPPORTED, "activation after the last layer");
     if (s->n_params <= 0 || (s->n_params & 3)) PINN_PLAN_FAIL(PINN_E_INVALID, "n_params must be a positive multiple of 4");
     if (s->nf < 0 || s->nf > PINN_MAX_DIRS || s->ns < 0 || s->ns > s->nf) PINN_PLAN_FAIL(PINN_E_INVALID, "jet set nf=%d ns=%d", s->nf, s->ns);
@@ -66,6 +69,10 @@ inline int build_dev_plan(const PinnSpec* s, DevPlan& h, int& fwd_rows, int& fwd
                     PINN_PLAN_FAIL(PINN_E_INVALID, "order %d: directions %d and %d coincide", s->order, e, d);
     }
     const int C = spec_channels(s);
+    // networks of k > 1 outputs (coupled systems): the thread kernel's second-order form only
+    if (n_out > 1 && (hi || s->nf > 4))
+        PINN_PLAN_FAIL(PINN_E_UNSUPPORTED, "a network of %d outputs with %s: only derivatives up to order 2 along at most 4 directions",
+                       n_out, hi ? "derivatives of order 3 / 4" : "more than 4 derivative directions");
     if (1 + C + s->n_vars > (int)(sizeof(s->eq_out) / sizeof(s->eq_out[0])))
         PINN_PLAN_FAIL(PINN_E_UNSUPPORTED, "%d jet channels + %d variables exceed the program's outputs", C, s->n_vars);
     if (s->has_ic && C * (1 + (s->ic_has_vars ? s->n_vars : 0)) > (int)(sizeof(s->ic_out) / sizeof(s->ic_out[0])))
@@ -82,12 +89,17 @@ inline int build_dev_plan(const PinnSpec* s, DevPlan& h, int& fwd_rows, int& fwd
         }
         if (!any) PINN_PLAN_FAIL(PINN_E_INVALID, "dir_vec[%d] is zero", d);
     }
-    if (s->n_slots < C || s->n_slots > PINN_MAX_SLOTS) PINN_PLAN_FAIL(PINN_E_INVALID, "n_slots %d", s->n_slots);
+    if (s->n_slots < C * n_out || s->n_slots > PINN_MAX_SLOTS) PINN_PLAN_FAIL(PINN_E_INVALID, "n_slots %d", s->n_slots);
     int rc;
     if ((rc = validate_prog(s->eq_prog, s->n_eq, s->n_slots, total, s->n_vars, "eq_prog", msg, msg_len))) return rc;
     if (s->has_ic && (rc = validate_prog(s->ic_prog, s->n_ic, s->n_slots, total, s->n_vars, "ic_prog", msg, msg_len))) return rc;
     for (int i = 0; i < 1 + C + s->n_vars; ++i)
         if (s->eq_out[i] < 0 || s->eq_out[i] >= s->n_slots) PINN_PLAN_FAIL(PINN_E_INVALID, "eq_out[%d]", i);
+    if (n_out > 1) {                                   // the partials of the k components: one contiguous block of k*C slots
+        if (s->eq_out[1] + C * n_out > s->n_slots) PINN_PLAN_FAIL(PINN_E_INVALID, "eq_out[1]: the partial block of %d slots ends past n_slots", C * n_out);
+        for (int c = 0; c < C; ++c)
+            if (s->eq_out[1 + c] != s->eq_out[1] + c) PINN_PLAN_FAIL(PINN_E_INVALID, "eq_out[%d] != eq_out[1] + %d", 1 + c, c);
+    }
     if (s->has_ic)
         for (int c = 0; c < C * (1 + (s->ic_has_vars ? s->n_vars : 0)); ++c)
             if (s->ic_out[c] < 0 || s->ic_out[c] >= s->n_slots) PINN_PLAN_FAIL(PINN_E_INVALID, "ic_out[%d]", c);

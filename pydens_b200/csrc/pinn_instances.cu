@@ -11,6 +11,7 @@
 #define PINN_WIDE 5          // wide_step_kernel, the tensor-core tile kernel
 #define PINN_SMALL 6         // small_step_kernel, the tiny-batch cluster kernel
 #define PINN_WIDE128 7       // wide_step_kernel of the 128-wide class
+#define PINN_COUPLED 8       // coupled_step_kernel, networks of 2..4 outputs
 
 #if PINN_UNIT == PINN_HI_JET
 #include "pinn_hi_kernel.cuh"
@@ -57,6 +58,11 @@ void enter() {
     kernel_slot(NF, J, 2).wide128 = wide::wide128_step_kernel<NF, J>;
 #elif PINN_UNIT == PINN_SMALL
     kernel_slot(NF, J, 2).small = small::small_step_kernel<NF, J>;
+#elif PINN_UNIT == PINN_COUPLED
+    using Cfg = VariantCfg<NF, J>;
+    CoupledSet& k = coupled_slot(NF, J);
+    k.step[0] = coupled_step_kernel<NF, J, false, Cfg::MAXT>;
+    k.step[1] = coupled_step_kernel<NF, J, true, Cfg::MAXT>;
 #else
 #error "PINN_UNIT names no kernel family"
 #endif

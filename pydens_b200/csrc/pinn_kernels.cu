@@ -40,11 +40,22 @@ const KernelSet* kernels(int nf, int ns, int order) {
     return k.step[1][1] ? &k : nullptr;
 }
 
+CoupledSet& coupled_slot(int nf, int ns) {
+    static CoupledSet table[5][5];                                     // [nf][ns]
+    return table[nf][ns];
+}
+
+const CoupledSet* coupled_kernels(int nf, int ns) {
+    if (nf < 0 || nf > 4 || ns < 0 || ns > nf) return nullptr;
+    const CoupledSet& k = coupled_slot(nf, ns);
+    return k.step[1] ? &k : nullptr;
+}
+
 // ---------------------------------------------------------------------------------------------------
-// Forward-only kernel (predict): u for explicit points.
+// Forward-only kernel (predict): u for explicit points; MULTI: the k components of every point, u_out [n_points, k].
 // ---------------------------------------------------------------------------------------------------
-template <bool GMEM>
-__global__ void __launch_bounds__(256, 1) forward_kernel(const __grid_constant__ DevPlan P, const FwdArgs a) {
+template <bool GMEM, bool MULTI>
+__device__ __forceinline__ void forward_body(const DevPlan& P, const FwdArgs& a) {
     extern __shared__ __align__(16) float smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
     const SmemLayout SL = smem_layout(P.weights_floats, 0, 0,
@@ -61,9 +72,25 @@ __global__ void __launch_bounds__(256, 1) forward_kernel(const __grid_constant__
         const long long pe = valid ? pl : a.n_points - 1;
         const float* src = a.points + (size_t)pe * P.total;
         for (int k = 0; k < P.total; ++k) st[k * RS] = __ldg(src + k);
-        float u = point_forward<16>(P, sw, a.params, st, RS, a.row_scr);
-        if (valid) a.u_out[pl] = u;
+        float u = point_forward<16, MULTI>(P, sw, a.params, st, RS, a.row_scr);
+        if constexpr (MULTI) {
+            const int k = P.layer[P.n_layers - 1].n_out;
+            for (int j = 0; j < k; ++j)
+                if (valid) a.u_out[(size_t)pl * k + j] = st[(size_t)(a.row_scr + j) * RS];
+        } else {
+            if (valid) a.u_out[pl] = u;
+        }
     }
+}
+
+template <bool GMEM>
+__global__ void __launch_bounds__(256, 1) forward_kernel(const __grid_constant__ DevPlan P, const FwdArgs a) {
+    forward_body<GMEM, false>(P, a);
+}
+
+template <bool GMEM>
+__global__ void __launch_bounds__(256, 1) coupled_forward_kernel(const __grid_constant__ DevPlan P, const FwdArgs a) {
+    forward_body<GMEM, true>(P, a);
 }
 
 // The forward-only form of the 128-wide tile kernel (declared in pinn_wide_kernel.cuh).
@@ -126,6 +153,7 @@ static int fail(int code, const char* fmt, ...) {
 // be real GEMMs.  *max_width: the widest hidden layer.
 static bool wide_eligible(const pinn::DevPlan& h, int* max_width) {
     if (h.n_layers < 2 || h.n_layers > pinn::wide::MAX_LAYERS) return false;
+    if (h.layer[h.n_layers - 1].n_out != 1) return false;           // networks of several outputs: thread kernel only
     int mw = 0;
     for (int l = 0; l < h.n_layers; ++l) {
         const pinn::DevLayer& L = h.layer[l];
@@ -150,7 +178,8 @@ struct PinnPlan {
     int small_smem;
     int wide_ctas;                           // CTAs the tile kernel runs on (<= sm_count)
     const KernelSet* ks;                     // the kernels of this plan's jet set
-    StepKernelFn fn_smem, fn_gmem;           // the pair matching this plan (plain or general)
+    StepKernelFn fn_smem, fn_gmem;           // the pair matching this plan (plain or general, or coupled_step_kernel)
+    bool coupled;                            // a network of 2..4 outputs: coupled_step_kernel / coupled_forward_kernel
     int sm_count;
     int smem_optin;
     // step kernel launch config
@@ -245,7 +274,9 @@ static int place_forward_kernel(PinnPlan* p) {
     else { p->fwd_gmem = true; SL = smem_layout(h.weights_floats, 0, 0, h.n_params); }
     p->fwd_threads = nw * 32; p->fwd_smem_bytes = SL.total_f * 4;
     if (p->fwd_smem_bytes > p->smem_optin - 64) return fail(PINN_E_UNSUPPORTED, "network too large for shared memory");
-    const cudaError_t e = allow_max_smem((const void*)(p->fwd_gmem ? forward_kernel<true> : forward_kernel<false>), p->smem_optin);
+    const void* fn = p->coupled ? (p->fwd_gmem ? (const void*)coupled_forward_kernel<true> : (const void*)coupled_forward_kernel<false>)
+                                : (p->fwd_gmem ? (const void*)forward_kernel<true> : (const void*)forward_kernel<false>);
+    const cudaError_t e = allow_max_smem(fn, p->smem_optin);
     if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(fwd): %s", cudaGetErrorString(e));
     return PINN_OK;
 }
@@ -343,7 +374,7 @@ extern "C" int pinn_plan_create(const PinnSpec* s, int device, PinnPlan** out) {
     if (!p) return fail(PINN_E_INVALID, "out of memory");
     {
         char msg[256];
-        const int rc = build_dev_plan(s, p->h, p->fwd_rows, p->fwd_row_scr, msg, sizeof(msg));
+        const int rc = build_dev_plan(s, p->h, p->fwd_rows, p->fwd_row_scr, msg, sizeof(msg), 4);
         if (rc) return fail(rc, "%s", msg);
     }
     // orders 3 / 4 take whole jets per direction (pinn_hi_kernel.cuh), one kernel per (nf, order); their plans have ns = 0
@@ -358,6 +389,14 @@ extern "C" int pinn_plan_create(const PinnSpec* s, int device, PinnPlan** out) {
     const int gen = p->h.general ? 1 : 0;
     p->fn_smem = p->ks->step[gen][0];
     p->fn_gmem = p->ks->step[gen][1] ? p->ks->step[gen][1] : p->ks->step[1][1];
+    // networks of 2..4 outputs: their own step kernels (build_dev_plan has refused what those do not cover)
+    p->coupled = p->h.layer[p->h.n_layers - 1].n_out > 1;
+    if (p->coupled) {
+        const CoupledSet* cs = coupled_kernels(p->h.nf, p->h.ns);
+        if (!cs) return fail(PINN_E_UNSUPPORTED, "no kernel for a network of several outputs with nf=%d ns=%d", p->h.nf, p->h.ns);
+        p->fn_smem = cs->step[0];
+        p->fn_gmem = cs->step[1];
+    }
     p->spec = *s;
     p->device = device;
 
@@ -375,8 +414,10 @@ extern "C" int pinn_plan_create(const PinnSpec* s, int device, PinnPlan** out) {
     int thread_rc = place_step_kernel(p.get());
     if (thread_rc == PINN_OK) thread_rc = place_forward_kernel(p.get());
     if (thread_rc != PINN_OK && thread_rc != PINN_E_UNSUPPORTED) return thread_rc;
-    place_multi_kernel(p.get());
-    place_small_kernel(p.get());
+    if (!p->coupled) {                           // the persistent multi-step kernels take networks of one output only
+        place_multi_kernel(p.get());
+        place_small_kernel(p.get());
+    }
     if (int rc = place_wide_kernel(p.get(), order, thread_rc)) return rc;
     *out = p.release();
     return PINN_OK;
@@ -805,8 +846,13 @@ extern "C" int pinn_forward(const PinnPlan* p, const float* params, const float*
     a.spill = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_spill_off(p));
     a.rows_total = p->fwd_rows; a.row_scr = p->fwd_row_scr;
     const int grid = grid_for(p, n_points, p->fwd_threads);
-    if (p->fwd_gmem) forward_kernel<true><<<grid, p->fwd_threads, p->fwd_smem_bytes, st>>>(p->h, a);
-    else             forward_kernel<false><<<grid, p->fwd_threads, p->fwd_smem_bytes, st>>>(p->h, a);
+    if (p->coupled) {
+        if (p->fwd_gmem) coupled_forward_kernel<true><<<grid, p->fwd_threads, p->fwd_smem_bytes, st>>>(p->h, a);
+        else             coupled_forward_kernel<false><<<grid, p->fwd_threads, p->fwd_smem_bytes, st>>>(p->h, a);
+    } else {
+        if (p->fwd_gmem) forward_kernel<true><<<grid, p->fwd_threads, p->fwd_smem_bytes, st>>>(p->h, a);
+        else             forward_kernel<false><<<grid, p->fwd_threads, p->fwd_smem_bytes, st>>>(p->h, a);
+    }
     CUDA_TRY(cudaGetLastError());
     return PINN_OK;
 }

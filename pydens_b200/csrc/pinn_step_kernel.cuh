@@ -432,8 +432,9 @@ __device__ __forceinline__ void cta_partial(const StepArgs& a, const float* wacc
 // ---------------------------------------------------------------------------------------------------
 // The fit-step kernel.
 // ---------------------------------------------------------------------------------------------------
-template <int NF, int NS, bool GMEM, int MAXT, int JF, bool GEN>
-__global__ void __launch_bounds__(MAXT, 1) step_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
+// The body of every thread-kernel step: MULTI selects the form for networks of 2..4 outputs (point_step).
+template <int NF, int NS, bool GMEM, int JF, bool GEN, bool MULTI>
+__device__ __forceinline__ void step_body(const DevPlan& P, const StepArgs& a) {
     extern __shared__ __align__(16) float smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
 
@@ -477,7 +478,7 @@ __global__ void __launch_bounds__(MAXT, 1) step_kernel(const __grid_constant__ D
             if (P.total > 4) b1 = philox_block(gidx, step, a.seed, 1u);
             for (int k = 0; k < P.total; ++k) st[k * RS] = sample_column(P.cols[k], k, gidx, step, a.seed, b0, b1);
         }
-        float r = point_step<NF, NS, JF, GEN>(P, sw, a.params, st, RS, valid, a.inv_n, sink, part);
+        float r = point_step<NF, NS, JF, GEN, MULTI>(P, sw, a.params, st, RS, valid, a.inv_n, sink, part);
         if (a.residual && valid) a.residual[pl] = r;
     }
 
@@ -500,6 +501,17 @@ __global__ void __launch_bounds__(MAXT, 1) step_kernel(const __grid_constant__ D
     // CTA partial -> global, then the last CTA folds all partials in block order
     cta_partial(a, wacc_all, n_out_floats, nwarps);
     finish_grid(a, n_out_floats);
+}
+
+template <int NF, int NS, bool GMEM, int MAXT, int JF, bool GEN>
+__global__ void __launch_bounds__(MAXT, 1) step_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
+    step_body<NF, NS, GMEM, JF, GEN, false>(P, a);
+}
+
+// The step of a network with 2..4 outputs (coupled systems): the general form, k read from the plan at run time.
+template <int NF, int NS, bool GMEM, int MAXT>
+__global__ void __launch_bounds__(MAXT, 1) coupled_step_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
+    step_body<NF, NS, GMEM, 16, true, true>(P, a);
 }
 
 
@@ -656,6 +668,14 @@ struct KernelSet {
     int maxt;                                // threads per CTA the step kernels are compiled for
     StepKernelFn wide128;                    // the tile kernel's class for hidden widths up to 128, 512 threads
 };
+
+// The step kernels of one jet set for networks of 2..4 outputs: coupled_step_kernel [GMEM].  Their own table, filled by
+// the 'coupled' build units; coupled_kernels(nf, ns) is nullptr outside 0 <= ns <= nf <= 4.
+struct CoupledSet {
+    StepKernelFn step[2];
+};
+const CoupledSet* coupled_kernels(int nf, int ns);
+CoupledSet& coupled_slot(int nf, int ns);
 
 // The set of a jet set, or nullptr when none was built: 0 <= ns <= nf <= PINN_MAX_DIRS for order 2; 1 <= nf <= 4 and
 // ns = 0 for orders 3 / 4 (their plans carry no second-order channels).  Defined in pinn_kernels.cu.

@@ -307,9 +307,11 @@ class FusedEngine:
         return out
 
     def forward(self, pts):
+        """ u at explicit points: [n] for a network of one output, [n, k] (row-major) for k outputs. """
         pts = pts.to(self.device, torch.float32).contiguous()
         n = pts.shape[0]
-        u = torch.empty(n, dtype=torch.float32, device=self.device)
+        k = self.solver._traced.n_out
+        u = torch.empty((n, k) if k > 1 else n, dtype=torch.float32, device=self.device)
         _native.check(self.lib.pinn_forward(self.plan, C.c_void_p(self.flat.data_ptr()), C.c_void_p(pts.data_ptr()),
                                             C.c_int64(n), C.c_void_p(u.data_ptr()),
                                             C.c_void_p(self.workspace.data_ptr()),

@@ -115,8 +115,8 @@ class Solver:
             chain = model.conv_block.dense_chain()
             if chain is None:
                 raise tracer.NotLowerable('layout %r is not a plain dense chain' % model.conv_block.layout)
-            if chain[-1][1] != 'none' or chain[-1][0].out_features != 1:
-                raise tracer.NotLowerable('network must end with a dense layer of one unit')
+            if chain[-1][1] != 'none' or not 1 <= chain[-1][0].out_features <= 4:
+                raise tracer.NotLowerable('network must end with a dense layer of one to four units')
             if chain[-1][2] is not None:
                 raise tracer.NotLowerable('skip connection into the output layer')
             if any(c[0].bias is None for c in chain) or len(chain) > _native.MAX_LAYERS:
@@ -138,7 +138,8 @@ class Solver:
 
             ic = model.raw_initial_condition
             self._traced = tracer.trace(self.equation, model.total, None, initial_condition=ic,
-                                        ndims_spatial=model.ndims_spatial, run=run, criterion=self._crit_key)
+                                        ndims_spatial=model.ndims_spatial, run=run, criterion=self._crit_key,
+                                        n_out=chain[-1][0].out_features)
             self._chain = chain
         except tracer.NotLowerable as exc:
             self._traced = None
@@ -164,7 +165,8 @@ class Solver:
         launch — one model evaluation at fixed points, combined pointwise — else None (autograd adds it). """
         if num not in self._traced_constraints:
             lowered = None
-            if self._traced is not None and os.environ.get('PYDENS_B200_FUSED_CONSTRAINTS') != '0':
+            # a network of several outputs: its constraints are added by autograd (the constraint programs are scalar)
+            if self._traced is not None and self._traced.n_out == 1 and os.environ.get('PYDENS_B200_FUSED_CONSTRAINTS') != '0':
                 model = self.model
                 try:
                     traced, args = tracer.trace_constraint(self.constraints[num], model.total,
@@ -385,13 +387,13 @@ class Solver:
 
     def predict(self, *xs):
         """ Solution approximation at the given points; every argument is a tensor / array / number,
-        tiled to the longest (reference :466-487).  Returns an (N x 1) numpy array. """
+        tiled to the longest (reference :466-487).  Returns an (N x k) numpy array for a network of k outputs. """
         pts = self.reshape_and_concat(xs).to(self.device, torch.float32)
         self.model.eval()
         if self._traced is not None and self.backend != 'torch' and self.device.type == 'cuda':
             engine = self._get_engine()
             if engine is not None:
-                return engine.forward(pts).reshape(-1, 1).cpu().numpy()
+                return engine.forward(pts).reshape(-1, self._traced.n_out).cpu().numpy()
         with torch.no_grad():
             result = self.ctx.run(self.model, pts)
         return result.detach().cpu().numpy()

@@ -58,6 +58,8 @@ class Expr:
             return 'x%d' % self.value
         if self.kind == 'u':
             return 'u' + ''.join('_%d' % i for i in self.value)
+        if self.kind == 'uc':
+            return 'u[%d]' % self.value[0] + ''.join('_%d' % i for i in self.value[1])
         if self.kind == 'var':
             return 'V[%s]' % self.value
         if self.kind == 'ch':
@@ -88,6 +90,11 @@ def coord(k):
 
 def uleaf(multi_index=()):
     return Expr('u', (), tuple(sorted(multi_index)))
+
+
+def ucleaf(j, multi_index=()):
+    """ Component j of the output of a network with several outputs, differentiated along `multi_index`. """
+    return Expr('uc', (), (int(j), tuple(sorted(multi_index))))
 
 
 def var(name):
@@ -270,6 +277,10 @@ def diff_coord(e, k, memo=None):
         if len(e.value) >= MAX_ORDER:
             raise NotLowerable('derivatives of order > %d are not supported by the fused path' % MAX_ORDER)
         r = uleaf(e.value + (k,))
+    elif e.kind == 'uc':
+        if len(e.value[1]) >= MAX_ORDER:
+            raise NotLowerable('derivatives of order > %d are not supported by the fused path' % MAX_ORDER)
+        r = ucleaf(e.value[0], e.value[1] + (k,))
     else:
         r = _chain(e, lambda a: diff_coord(a, k, memo))
     memo[e] = r
@@ -284,7 +295,7 @@ def diff_leaf(e, leaf, memo=None):
         return hit
     if e is leaf:
         r = ONE
-    elif e.kind in ('const', 'coord', 'u', 'var', 'ch'):
+    elif e.kind in ('const', 'coord', 'u', 'uc', 'var', 'ch'):
         r = ZERO
     else:
         r = _chain(e, lambda a: diff_leaf(a, leaf, memo))
@@ -395,7 +406,7 @@ def _clamp(a, lo=None, hi=None):
     return a
 
 
-_FINITE_KINDS = ('const', 'coord', 'u', 'var', 'ch', 'add', 'sub', 'mul', 'neg', 'sin', 'cos', 'tanh', 'sigmoid', 'abs', 'sign')
+_FINITE_KINDS = ('const', 'coord', 'u', 'uc', 'var', 'ch', 'add', 'sub', 'mul', 'neg', 'sin', 'cos', 'tanh', 'sigmoid', 'abs', 'sign')
 
 
 def _always_finite(e, seen=None):
@@ -653,7 +664,7 @@ def _as_column(s):
     """ `s` when it stands for an [N, 1] column of the batch: an expression of u or of the point columns.  A V(...)
     variable is a one-element tensor and a constant a number in the reference; indexing, splitting or concatenating
     those fails there (or means something else), so it is not lowered here either. """
-    if not leaves(s.expr, ('u', 'coord')):
+    if not leaves(s.expr, ('u', 'uc', 'coord')):
         raise NotLowerable('indexing / split / concatenation of a traced value that is not a column of the batch')
     return s
 
@@ -754,10 +765,69 @@ class VecSym:
     __array_ufunc__ = None
 
 
+class Components:
+    """ Symbolic stand-in for the `[N, k]` output of a network with k = 2..4 outputs (coupled systems).  The equation
+    picks component j as a column, with the forms that keep the [N, 1] shape: f[:, j:j+1], f[:, [j]], f[..., j:j+1],
+    torch.split(f, 1, dim=1), torch.chunk(f, k, dim=1) and their tensor-method spellings.  Anything else done to the whole
+    value — arithmetic, D(), f[:, j] (one-dimensional in torch) — stays on autograd. """
+
+    def __init__(self, k):
+        self.k = k
+
+    def column(self, j):
+        if not 0 <= j < self.k:
+            raise NotLowerable('component %d of a network with %d outputs' % (j, self.k))
+        return Sym(ucleaf(j))
+
+    def __getitem__(self, key):
+        if not isinstance(key, tuple) or len(key) != 2 or not (key[0] is Ellipsis or key[0] == slice(None)):
+            raise NotLowerable('indexing the network output other than f[:, j:j+1] / f[:, [j]]')
+        sel = key[1]
+        if isinstance(sel, slice) and sel.step in (None, 1) and isinstance(sel.start, int) and isinstance(sel.stop, int) \
+                and sel.start >= 0 and sel.stop == sel.start + 1:
+            return self.column(sel.start)
+        if isinstance(sel, list) and len(sel) == 1 and isinstance(sel[0], int) and sel[0] >= 0:
+            return self.column(sel[0])
+        raise NotLowerable('indexing the network output other than f[:, j:j+1] / f[:, [j]] (f[:, j] is one-dimensional)')
+
+    def split(self, size, dim=None):
+        _column_dim(dim)
+        if not (size == 1 or isinstance(size, (list, tuple)) and list(size) == [1] * self.k):
+            raise NotLowerable('torch.split of the network output with sizes %r (one column per piece only)' % (size,))
+        return tuple(self.column(j) for j in range(self.k))
+
+    def chunk(self, chunks, dim=None):
+        _column_dim(dim)
+        if not (isinstance(chunks, int) and chunks >= self.k):
+            raise NotLowerable('torch.chunk of the network output into %r chunks (one column per chunk only)' % (chunks,))
+        return tuple(self.column(j) for j in range(self.k))
+
+    @classmethod
+    def __torch_function__(cls, func, types, args=(), kwargs=None):
+        name = getattr(func, '__name__', None)
+        if name in ('split', 'chunk') and args and isinstance(args[0], Components):
+            return getattr(args[0], name)(*args[1:], **(kwargs or {}))
+        raise NotLowerable('torch.%s of the whole output of a network with several outputs' % name)
+
+    def __getattr__(self, name):
+        if name.startswith('__'):
+            raise AttributeError(name)
+        raise NotLowerable('%r of the whole output of a network with several outputs' % name)
+
+    def _unsupported(self, *args, **kwargs):
+        raise NotLowerable('arithmetic on the whole output of a network with several outputs (select a component first)')
+
+    __add__ = __radd__ = __sub__ = __rsub__ = __mul__ = __rmul__ = __truediv__ = __rtruediv__ = _unsupported
+    __pow__ = __rpow__ = __neg__ = __pos__ = __abs__ = __len__ = __iter__ = __bool__ = _unsupported
+    __array_ufunc__ = None
+
+
 def sym_D(y, x):
     """ Symbolic counterpart of the D token. """
     if isinstance(y, VecSym):
         raise NotLowerable('D() of a residual with several columns')
+    if isinstance(y, Components):
+        raise NotLowerable('D() of the whole output of a network with several outputs (select a component first)')
     if not isinstance(x, Sym) or x.expr.kind != 'coord':
         raise NotLowerable('D(y, x): x must be one of the equation arguments')
     return Sym(diff_coord(_as_expr(y), x.expr.value))
@@ -784,11 +854,12 @@ class Program:
         return len(self.instrs)
 
 
-def lower(outputs, channel_of_u, var_index, n_reserved):
+def lower(outputs, channel_of_u, var_index, n_reserved, pinned=None):
     """ Linearise `outputs` (list of Expr) into one program.
 
     Slots [0, n_reserved) hold the jet of u on entry and are never written ('ch' leaves read them;
     `channel_of_u` is kept for the signature only); `var_index` maps a variable name to its VAR operand.
+    `pinned`: expressions to compute straight into a given reserved slot instead of a scratch one.
     """
     order, seen = [], set()
 
@@ -854,7 +925,7 @@ def lower(outputs, channel_of_u, var_index, n_reserved):
         if e.kind == 'ch':
             slot_of[e] = e.value
             continue
-        if e.kind == 'u':
+        if e.kind in ('u', 'uc'):
             raise NotLowerable('unexpected derivative leaf %r' % e)
         imm = immediate_form(e)
         operands = [imm[1]] if imm else list(e.args)
@@ -863,7 +934,7 @@ def lower(outputs, channel_of_u, var_index, n_reserved):
         for a in operands:
             if last_use.get(a) == i and a.kind != 'ch' and slot_of[a] >= n_reserved and slot_of[a] not in free:
                 free.append(slot_of[a])
-        dst = alloc()
+        dst = pinned[e] if pinned and e in pinned else alloc()
         slot_of[e] = dst
         if e.kind == 'const':
             instrs.append((OP['CONST'], dst, 0, 0, e.value))
@@ -932,6 +1003,7 @@ class TracedEquation:
         self.ic_prog = None         # outputs: jet of ic (C entries) [+ C partials per variable] or None
         self.ic_has_vars = False
         self.n_slots = 0
+        self.n_out = 1              # outputs of the network (k); k > 1: see trace
         self.order = 2              # 3 / 4: every direction carries its whole Taylor jet up to this order (ns = 0):
                                     # channel 1 + d*order + (k-1) = k-th derivative along direction d
 
@@ -1041,27 +1113,33 @@ def _leaves_of(exprs, kinds):
     return found
 
 
-def trace(equation, total, var_factory, initial_condition=None, ndims_spatial=0, run=None, criterion=None):
+def trace(equation, total, var_factory, initial_condition=None, ndims_spatial=0, run=None, criterion=None, n_out=1):
     """ Trace `equation(u, *xs)` (and `initial_condition(*x_spatial)` if callable).
 
     `var_factory(name)` is installed by the caller so that V(name, ...) returns `Sym(var(name))`
     during the trace.  `run` wraps the call (the Solver passes its contextvars ctx.run).
     `criterion`: see apply_criterion (default: the residual itself, MSE).
     The equation may return one column or several (`torch.cat([...], dim=1)`): see residual_outputs.
+    `n_out` = k in 2..4: the network has k outputs; the equation selects component j (Components), every component
+    carries the same jet set, and the residual program follows the k-output convention of include/pinn_b200.h: slot
+    j*C + c holds channel c of component j on entry, and dr/d(that channel) is left in slot eq_out[1] + j*C + c.
     """
     run = run or (lambda f, *a: f(*a))
     xs = [Sym(coord(k)) for k in range(total)]
-    rs = _residual_columns(run(equation, Sym(uleaf()), *xs))
+    rs = _residual_columns(run(equation, Sym(uleaf()) if n_out == 1 else Components(n_out), *xs))
     res = rs[0]
     T = TracedEquation()
     T.residual = res
+    T.n_out = n_out
 
-    u_leaves = _leaves_of(rs, ('u',))
-    if any(len(l.value) > 2 for l in u_leaves):
+    u_leaves = _leaves_of(rs, ('u',) if n_out == 1 else ('uc',))
+    mis = [l.value for l in u_leaves] if n_out == 1 else [l.value[1] for l in u_leaves]
+    if any(len(mi) > 2 for mi in mis):
+        if n_out > 1:
+            raise NotLowerable('derivatives of order > 2 of a network with several outputs')
         return _trace_high_order(T, rs, u_leaves, xs, total, initial_condition, ndims_spatial, run, criterion)
     first, second, mixed = set(), set(), set()
-    for l in u_leaves:
-        mi = l.value
+    for mi in mis:
         if len(mi) == 1:
             first.add(mi[0])
         elif len(mi) == 2:
@@ -1081,27 +1159,34 @@ def trace(equation, total, var_factory, initial_condition=None, ndims_spatial=0,
     nf, ns = len(T.dirs), T.ns
     if nf > MAX_DIRS:
         raise NotLowerable('more than %d derivative directions' % MAX_DIRS)
+    if n_out > 1 and nf > 4:
+        raise NotLowerable('more than 4 derivative directions in a network with several outputs')
     if nf > 4:
         # five / six directions (full Hessians in 3-D, Laplacians in 5-D / 6-D): the library holds ONE kernel per
         # direction count there, the one in which every direction carries its second derivative — first-order-only
         # directions are promoted (their second-order channel is computed and meets a zero adjoint seed)
         T.ns = ns = nf
     C = 1 + nf + ns
-    mapping = {uleaf(): chleaf(0)}
-    for d, col in enumerate(T.dirs):
-        if col >= 0:
-            mapping[uleaf((col,))] = chleaf(1 + d)
-            if d < ns:
-                mapping[uleaf((col, col))] = chleaf(1 + nf + d)
-    for n, (i, j) in enumerate(mixed):
-        d = len(axes2) + n
-        mapping[uleaf((i, j))] = mul(const(0.5), sub(sub(chleaf(1 + nf + d), mapping[uleaf((i, i))]),
-                                                     mapping[uleaf((j, j))]))
+    mapping = {}
+    for q in range(n_out):                         # component q's jet: slots q*C .. q*C + C-1
+        def leaf(mi=(), q=q):
+            return uleaf(mi) if n_out == 1 else ucleaf(q, mi)
+        base = q * C
+        mapping[leaf()] = chleaf(base)
+        for d, col in enumerate(T.dirs):
+            if col >= 0:
+                mapping[leaf((col,))] = chleaf(base + 1 + d)
+                if d < ns:
+                    mapping[leaf((col, col))] = chleaf(base + 1 + nf + d)
+        for n, (i, j) in enumerate(mixed):
+            d = len(axes2) + n
+            mapping[leaf((i, j))] = mul(const(0.5), sub(sub(chleaf(base + 1 + nf + d), mapping[leaf((i, i))]),
+                                                        mapping[leaf((j, j))]))
     memo = {}
     rs = [substitute(r, mapping, memo) for r in rs]
     res = rs[0]
     chan = {}
-    by_channel = {c: chleaf(c) for c in range(C)}
+    by_channel = {c: chleaf(c) for c in range(n_out * C)}
 
     # the initial condition is traced first: its variables join the equation's (README.md:112-118)
     ic = None
@@ -1119,9 +1204,9 @@ def trace(equation, total, var_factory, initial_condition=None, ndims_spatial=0,
         raise NotLowerable('more than 4 trainable variables')
     var_index = {n: i for i, n in enumerate(T.var_names)}
 
-    outputs = residual_outputs(rs, [by_channel[c] for c in range(C)] + [var(n) for n in T.var_names], criterion)
+    outputs = residual_outputs(rs, [by_channel[c] for c in range(n_out * C)] + [var(n) for n in T.var_names], criterion)
     T.residual = apply_criterion(res, criterion) if len(rs) == 1 else outputs[0]
-    T.eq_prog = lower(outputs, chan, var_index, C)
+    T.eq_prog = lower(outputs, chan, var_index, C) if n_out == 1 else _lower_partial_block(outputs, var_index, C, n_out)
     T.n_slots = T.eq_prog.n_slots
 
     if ic is not None:
@@ -1143,6 +1228,23 @@ def trace(equation, total, var_factory, initial_condition=None, ndims_spatial=0,
         T.ic_prog = lower(jet, {}, var_index, base)
         T.n_slots = max(T.n_slots, T.ic_prog.n_slots)
     return T
+
+
+def _lower_partial_block(outputs, var_index, C, n_out):
+    """ The residual program of a network with k = n_out outputs: `outputs` = [r, dr/d(slot s) for s < k C, dr/dV ..].
+    The k C partials must form one contiguous block: slots [k C, 2 k C) are kept out of the lowering and filled by copies
+    (x * 1, exact) at the end where a partial is not computed in its block slot in the first place.  Program outputs as in a one-output program: [r, the block's first C slots, dr/dV ..]. """
+    kc = n_out * C
+    pinned = {}
+    for s in range(kc):                            # a partial met for the first time is computed in its block slot
+        e = outputs[1 + s]
+        if e.kind != 'ch' and e not in pinned and e is not outputs[0] and all(e is not o for o in outputs[1 + kc:]):
+            pinned[e] = kc + s
+    prog = lower(outputs, {}, var_index, 2 * kc, pinned)
+    instrs = prog.instrs + [(OP['MULI'], kc + s, prog.outs[1 + s], 0, 1.0) for s in range(kc) if prog.outs[1 + s] != kc + s]
+    if len(instrs) > MAX_PROG:
+        raise NotLowerable('expression needs %d instructions (max %d)' % (len(instrs), MAX_PROG))
+    return Program(instrs, [prog.outs[0]] + [kc + c for c in range(C)] + prog.outs[1 + kc:], prog.n_slots)
 
 
 def _trace_high_order(T, rs, u_leaves, xs, total, initial_condition, ndims_spatial, run, criterion=None):

@@ -40,8 +40,11 @@ def main():
     else:                                  # a registry problem, e.g. wave3d: the tensor-core tile kernel under data parallelism
         import problems as P
         import problems_wide as PW         # ... or a 128-wide network (poisson_wide128)
+        import problems_coupled as PC      # ... or a network of several outputs (navier_stokes2d)
         if problem in PW.PROBLEMS:
             P = PW
+        elif problem in PC.PROBLEMS:
+            P = PC
         cfg = P.PROBLEMS[problem]
         solver = Solver(P.bind(problem, D, lambda n, init: V(n, data=torch.Tensor([init]))), ndims=cfg['ndims'],
                         nparams=cfg['nparams'], initial_condition=cfg['ic'], boundary_condition=cfg['bc'],
