@@ -5,7 +5,7 @@
 // hand-derived reverse sweep).  The functions are `__host__ __device__` so the very same code
 // can be compiled by g++ into the test-only emulation harness (tests/emul/) and checked against
 // the fp64 oracle on a machine without a GPU.  Cross-lane work (the weight-gradient reduction)
-// is isolated in emit_entries().
+// is isolated in emit_entries() / emit_entries_perm().
 //
 // Reference semantics being reproduced (analysiscenter/pydens, pydens/model_torch.py):
 //   forward  :170-172 (MLP via batchflow Block) + anzatc :107-128
@@ -44,6 +44,32 @@ inline float2 make_float2(float x, float y) { float2 r; r.x = x; r.y = y; return
 #define PINN_FMUL2(a2, s)     make_float2((a2).x * (s), (a2).y * (s))
 #define PINN_FFMA2V(a2, b2, c2) make_float2(fmaf((a2).x, (b2).x, (c2).x), fmaf((a2).y, (b2).y, (c2).y))
 #define PINN_FMUL2V(a2, b2)     make_float2((a2).x * (b2).x, (a2).y * (b2).y)
+
+// Phase clock, for measurement builds only (-DPINN_PHASE_CLOCK, compiled by tools/phase_clock.py; never by build()):
+// the thread-kernel step adds each warp's clock64() cycles per phase into pinn_phase_cycles (lane 0 adds, atomically).
+// The reverse phase of linear layer l is slot PINN_PHASE_REV + l (layer 0: its weight gradients); the butterflies are
+// counted inside the reverse phases as well.
+#define PINN_PHASE_LOAD 0          // the tile's coordinates into per-point storage
+#define PINN_PHASE_FWD 1           // forward through all layers
+#define PINN_PHASE_PROG 2          // ansatz, residual program and their adjoints
+#define PINN_PHASE_BFLY 3          // weight-gradient butterflies
+#define PINN_PHASE_TAIL 4          // after the last tile: warp sums, CTA partial, grid fold and Adam
+#define PINN_PHASE_REV 5
+#define PINN_PHASE_SLOTS (PINN_PHASE_REV + PINN_MAX_LAYERS)
+#if defined(PINN_PHASE_CLOCK)
+static __device__ unsigned long long pinn_phase_cycles[PINN_PHASE_SLOTS];
+#endif
+#if defined(PINN_PHASE_CLOCK) && defined(__CUDA_ARCH__)
+#define PINN_PHASE_T0(t) const long long t = clock64()
+#define PINN_PHASE_ADD(slot, t)                                                                              \
+    do {                                                                                                     \
+        const long long t_end_ = clock64();                                                                  \
+        if ((threadIdx.x & 31) == 0) atomicAdd(&pinn_phase_cycles[slot], (unsigned long long)(t_end_ - (t))); \
+    } while (0)
+#else
+#define PINN_PHASE_T0(t) do {} while (0)
+#define PINN_PHASE_ADD(slot, t) do {} while (0)
+#endif
 
 namespace pinn {
 
@@ -894,6 +920,50 @@ PINN_HD void emit_entries(float (&v)[NV], AddFn&& add) {
 #endif
 }
 
+// The select-free form of the butterfly.  Lane L keeps entry e in slot e ^ entry_perm<NV, LOW>() = e ^ (L % NV & ~(LOW - 1)):
+// at every stage S >= LOW each lane keeps slots [0, S), sends slots [S, 2S) and adds what its partner sent, and the
+// partner's slot i + S holds the same entry as the lane's slot i; the stages S < LOW, whose entries the caller keeps in
+// logical order, are warp_transpose_stage's.  A total depends only on the tree of lane distances (16, 8, 4, 2, 1), not on
+// the lane that ends up holding it, so the sums are bit-identical to warp_transpose_reduce's, without its two selects per
+// shuffle in the stages S >= LOW.  The callers fill the slots in this order: the per-point rows are one column per lane,
+// so a lane-dependent row is still one access per bank.  The host emulation is one lane: entry_perm is 0 there.
+template <int NV, int LOW = 1>
+PINN_HD int entry_perm() {
+#if defined(__CUDA_ARCH__)
+    return threadIdx.x & (NV - 1) & ~(LOW - 1);
+#else
+    return 0;
+#endif
+}
+
+#if defined(__CUDA_ARCH__)
+template <int S, int NV, int LOW>
+__device__ __forceinline__ void warp_xor_stage(float (&v)[NV], int lane) {
+    if constexpr (S < LOW && S < NV) {
+        warp_transpose_stage<S, NV>(v, lane);         // it runs the stages below S as well
+    } else {
+#pragma unroll
+        for (int i = 0; i < (S >= NV ? NV : S); ++i) v[i] += __shfl_xor_sync(0xffffffffu, v[S >= NV ? i : i + S], S);
+        if constexpr (S > 1) warp_xor_stage<S / 2, NV, LOW>(v, lane);
+    }
+}
+#endif
+
+template <int NV, int LOW = 1, class AddFn>
+PINN_HD void emit_entries_perm(float (&v)[NV], AddFn&& add) {
+    static_assert(NV >= 1 && NV <= 32 && (NV & (NV - 1)) == 0, "NV must be a power of two up to 32");
+    static_assert(LOW >= 1 && LOW <= NV && (LOW & (LOW - 1)) == 0, "LOW must be a power of two up to NV");
+#if defined(__CUDA_ARCH__)
+    PINN_PHASE_T0(t0);
+    const int lane = threadIdx.x & 31;
+    warp_xor_stage<16, NV, LOW>(v, lane);
+    if (lane < NV) add(lane, v[0]);
+    PINN_PHASE_ADD(PINN_PHASE_BFLY, t0);
+#else
+    for (int e = 0; e < NV; ++e) add(e, v[e]);
+#endif
+}
+
 struct GradSink {
     float* wacc;        // this warp's own accumulator in params layout (+ loss slot): no other warp writes it
     int dump;           // index of a scratch slot of the accumulator that swallows masked-off entries
@@ -916,15 +986,16 @@ struct GradSink {
 template <int NF, int NS>
 PINN_HD void bias_grad(const DevLayer& L, const float* __restrict__ out_rows, int RS, const GradSink& sink) {
     constexpr int C = 1 + NF + NS;
+    const int pe = entry_perm<32>();
 #pragma unroll 1
     for (int j0 = 0; j0 < L.n_out; j0 += 32) {
         float v[32];
 #pragma unroll
         for (int i = 0; i < 32; ++i) {
-            const int j = j0 + i < L.n_out ? j0 + i : L.n_out - 1;
+            const int j = j0 + (i ^ pe) < L.n_out ? j0 + (i ^ pe) : L.n_out - 1;
             v[i] = out_rows[(size_t)j * C * RS];
         }
-        emit_entries<32>(v, [&](int e, float t) {
+        emit_entries_perm<32>(v, [&](int e, float t) {
             sink.add_if(j0 + e < L.n_out, L.b_off + j0 + e, t);
         });
     }
@@ -934,9 +1005,14 @@ PINN_HD void bias_grad(const DevLayer& L, const float* __restrict__ out_rows, in
 //   weight AND bias gradients of L (the bias is normally column n_in of the same reduction batches: its
 //   "input jet" is (1, 0, …)) and — fused in the same loop — the adjoints of the layer below, pushed
 //   through that layer's activation and written over its stored jet in place.
-// JJ = output units per reduction batch (4 normally, 1 for the single-output top layer).
+// JJ = output units per reduction batch (4 normally, 1 for the single-output top layer, which takes 16 input columns
+// per block instead of 8 so that one 16-entry butterfly replaces two 8-entry ones).
 // No guards in the inner loops: rows/columns past the end are read from clamped (valid) addresses,
 // meet zero-padded weights, and their reduction entries are dropped at the sink.
+// Butterfly slots (emit_entries_perm with LOW = JJ): entry e = (m - m0) * JJ + (j - j0), and this lane's slot s * JJ + jj
+// holds entry (j0 + jj, m0 + (s ^ pm)).  Only the post jets are loaded in that order; the adjoint rows stay in logical
+// order, so the data gradient keeps its summation order over j and its broadcast weight rows, and one read of a row
+// serves both products.  The JJ entries of a column are reduced by the last log2(JJ) stages, with selects.
 template <int NF, int NS, int JJ, bool SKIP, bool GEN = SKIP>
 PINN_HD void bwd_layer(const DevLayer& L, int below_act_id, const float* __restrict__ sw,
                        const float* __restrict__ out_rows, float* __restrict__ in_rows, int RS,
@@ -946,7 +1022,8 @@ PINN_HD void bwd_layer(const DevLayer& L, int below_act_id, const float* __restr
                        float* __restrict__ adj_out /* where to stash the adjoint of a residual layer, or null */,
                        float* __restrict__ dump_rows /* C rows that swallow the stores of masked-off units */) {
     constexpr int C = 1 + NF + NS;
-    constexpr int JB = 8;
+    constexpr int JB = JJ == 1 ? 16 : 8;
+    const int pm = entry_perm<JJ * JB, JJ>() / JJ;
     const float* W = sw + L.w_s;
     const ActC below = make_actc(below_act_id);
     const ActC load_act = make_actc(SKIP ? load_act_id : below_act_id);
@@ -957,11 +1034,11 @@ PINN_HD void bwd_layer(const DevLayer& L, int below_act_id, const float* __restr
     const int n_cols = L.n_in + (fold_bias ? 1 : 0);
 #pragma unroll 1
     for (int m0 = 0; m0 < n_cols; m0 += JB) {
-        // neighbouring input units are kept as pairs
+        // input units are kept as pairs: those of butterfly slots 2h and 2h + 1
         float2 post[JB / 2][C];
 #pragma unroll
         for (int h = 0; h < JB / 2; ++h) {
-            const int ma = m0 + 2 * h, mb = ma + 1;
+            const int ma = m0 + ((2 * h) ^ pm), mb = m0 + ((2 * h + 1) ^ pm);
             const int ca = ma < L.n_in ? ma : L.n_in - 1, cb = mb < L.n_in ? mb : L.n_in - 1;
             load_post_jet2<NF, NS, GEN>(load_rows + (size_t)ca * C * RS, load_rows + (size_t)cb * C * RS, RS, load_act,
                                    post[h]);
@@ -994,7 +1071,7 @@ PINN_HD void bwd_layer(const DevLayer& L, int below_act_id, const float* __restr
 
         constexpr int BUNR = (C >= 8) ? PINN_BWD_UNR_WIDE : 1;
 #pragma unroll BUNR
-        for (int j0 = 0; j0 < L.n_out; j0 += JJ) {
+        for (int j0 = 0; j0 < (JJ == 1 ? 1 : L.n_out); j0 += JJ) {       // JJ == 1 only for n_out == 1
             float v[JJ * JB];
 #pragma unroll
             for (int jj = 0; jj < JJ; ++jj) {
@@ -1004,10 +1081,16 @@ PINN_HD void bwd_layer(const DevLayer& L, int below_act_id, const float* __restr
                 float zb[C];
 #pragma unroll
                 for (int c = 0; c < C; ++c) zb[c] = row[(size_t)c * RS];
+                // JB = 16 reads 16 floats from row j of [n_out_p4][n_in_p8]: for the single-output layer the columns
+                // past its row are the zero rows 1..3 of the padding, and they meet masked-off units only
                 const float4* wrow = reinterpret_cast<const float4*>(W + (size_t)j * L.n_in_p8 + m0);
-                const float4 w0 = wrow[0], w1 = wrow[1];
-                const float2 w[JB / 2] = {make_float2(w0.x, w0.y), make_float2(w0.z, w0.w),
-                                          make_float2(w1.x, w1.y), make_float2(w1.z, w1.w)};
+                float2 w[JB / 2];
+#pragma unroll
+                for (int q = 0; q < JB / 4; ++q) {
+                    const float4 wq = wrow[q];
+                    w[2 * q] = make_float2(wq.x, wq.y);
+                    w[2 * q + 1] = make_float2(wq.z, wq.w);
+                }
 #pragma unroll
                 for (int h = 0; h < JB / 2; ++h) {
                     float2 e = PINN_FMUL2(post[h][0], zb[0]);
@@ -1016,12 +1099,12 @@ PINN_HD void bwd_layer(const DevLayer& L, int below_act_id, const float* __restr
                         acc[h][c] = PINN_FFMA2(w[h], zb[c], acc[h][c]);
                         if (c > 0) e = PINN_FFMA2(post[h][c], zb[c], e);
                     }
-                    v[jj * JB + 2 * h] = e.x;
-                    v[jj * JB + 2 * h + 1] = e.y;
+                    v[2 * h * JJ + jj] = e.x;
+                    v[(2 * h + 1) * JJ + jj] = e.y;
                 }
             }
-            emit_entries<JJ * JB>(v, [&](int e, float t) {
-                const int j = j0 + e / JB, m = m0 + e % JB;
+            emit_entries_perm<JJ * JB, JJ>(v, [&](int e, float t) {
+                const int j = j0 + e % JJ, m = m0 + e / JJ;
                 sink.add_if(j < L.n_out && m <= L.n_in, m < L.n_in ? L.w_off + j * L.n_in + m : L.b_off + j, t);
             });
         }
@@ -1054,48 +1137,52 @@ PINN_HD void bwd_layer(const DevLayer& L, int below_act_id, const float* __restr
 }
 
 // Weight (and bias) gradients of the FIRST linear layer: its input jet is (x, e_dir, 0); the bias rides
-// in column n_in when n_in < PINN_MAX_DIMS.
-template <int NF, int NS>
+// in column n_in when n_in < MC.  MC = columns per output unit in a butterfly: PINN_MAX_DIMS, or 4 when
+// n_in + 1 <= 4 (two 8 x 4 butterflies cover 16 output units where 4 x 8 ones need four).  Slot jj * MC + s of this
+// lane holds entry (j0 + (jj ^ pj), s ^ pm) (emit_entries_perm).
+template <int NF, int NS, int MC>
 PINN_HD void wgrad_input_layer(const DevLayer& L, const float* __restrict__ out_rows,
                                const float* __restrict__ coords, int RS, const float* __restrict__ dirv,
                                const GradSink& sink) {
+    static_assert(MC == 4 || MC == PINN_MAX_DIMS, "4 or PINN_MAX_DIMS columns");
     constexpr int C = 1 + NF + NS;
-    float2 x[PINN_MAX_DIMS / 2];
-    float2 dv[NF > 0 ? NF : 1][PINN_MAX_DIMS / 2];
+    constexpr int JR = 32 / MC;                       // output units per butterfly
+    const int pe = entry_perm<32>(), pm = pe % MC, pj = pe / MC;
+    float2 x[MC / 2];
+    float2 dv[NF > 0 ? NF : 1][MC / 2];
 #pragma unroll
-    for (int h = 0; h < PINN_MAX_DIMS / 2; ++h) {
-        const int ma = 2 * h, mb = 2 * h + 1;
+    for (int h = 0; h < MC / 2; ++h) {
+        const int ma = (2 * h) ^ pm, mb = (2 * h + 1) ^ pm;
         x[h] = make_float2((ma < L.n_in) ? coords[(size_t)ma * RS] : (ma == L.n_in ? 1.0f : 0.0f),
                            (mb < L.n_in) ? coords[(size_t)mb * RS] : (mb == L.n_in ? 1.0f : 0.0f));
 #pragma unroll
         for (int d = 0; d < NF; ++d) dv[d][h] = make_float2(dirv[d * PINN_MAX_DIMS + ma], dirv[d * PINN_MAX_DIMS + mb]);
     }
 #pragma unroll 1
-    for (int j0 = 0; j0 < L.n_out; j0 += 4) {
-        float v[4 * PINN_MAX_DIMS];
+    for (int j0 = 0; j0 < L.n_out; j0 += JR) {
+        float v[32];
 #pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-            const int j = j0 + jj < L.n_out ? j0 + jj : L.n_out - 1;
+        for (int jj = 0; jj < JR; ++jj) {
+            const int j = j0 + (jj ^ pj) < L.n_out ? j0 + (jj ^ pj) : L.n_out - 1;
             const float* row = out_rows + (size_t)j * C * RS;
             float zb[1 + NF];
 #pragma unroll
             for (int c = 0; c < 1 + NF; ++c) zb[c] = row[(size_t)c * RS];
 #pragma unroll
-            for (int h = 0; h < PINN_MAX_DIMS / 2; ++h) {
+            for (int h = 0; h < MC / 2; ++h) {
                 float2 e = PINN_FMUL2(x[h], zb[0]);
 #pragma unroll
                 for (int d = 0; d < NF; ++d) e = PINN_FFMA2(dv[d][h], zb[1 + d], e);
-                v[jj * PINN_MAX_DIMS + 2 * h] = e.x;
-                v[jj * PINN_MAX_DIMS + 2 * h + 1] = e.y;
+                v[jj * MC + 2 * h] = e.x;
+                v[jj * MC + 2 * h + 1] = e.y;
             }
         }
-        emit_entries<4 * PINN_MAX_DIMS>(v, [&](int e, float t) {
-            const int j = j0 + e / PINN_MAX_DIMS, m = e % PINN_MAX_DIMS;
-            sink.add_if(j < L.n_out && m <= L.n_in && m < PINN_MAX_DIMS,
-                        m < L.n_in ? L.w_off + j * L.n_in + m : L.b_off + j, t);
+        emit_entries_perm<32>(v, [&](int e, float t) {
+            const int j = j0 + e / MC, m = e % MC;
+            sink.add_if(j < L.n_out && m <= L.n_in, m < L.n_in ? L.w_off + j * L.n_in + m : L.b_off + j, t);
         });
     }
-    if (L.n_in >= PINN_MAX_DIMS) bias_grad<NF, NS>(L, out_rows, RS, sink);
+    if (L.n_in >= MC) bias_grad<NF, NS>(L, out_rows, RS, sink);
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -1136,6 +1223,7 @@ PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weigh
     float* scr = st + (size_t)P.row_scr * RS;
 
     // ---- forward through the hidden layers (and, for k outputs, the output layer: its k jets go to storage) ----
+    PINN_PHASE_T0(t_fwd);
 #pragma unroll 1
     for (int l = 0; l + (MULTI ? 0 : 1) < Ln; ++l) {
         const DevLayer& L = P.layer[l];
@@ -1152,8 +1240,10 @@ PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weigh
         const float* in_rows = (Ln == 1) ? coords : layer_output<GEN>(P, Ln - 2, units, C, RS, in_act);
         fwd_final<NF, NS, GEN>(L, sw, in_rows, Ln == 1, in_act, &P.dir_vec[0][0], RS, N);
     }
+    PINN_PHASE_ADD(PINN_PHASE_FWD, t_fwd);
 
     // ---- ansatz + residual ----
+    PINN_PHASE_T0(t_prog);
     float icj[C];
 #pragma unroll
     for (int c = 0; c < C; ++c) icj[c] = 0.0f;
@@ -1220,8 +1310,10 @@ PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weigh
 #pragma unroll
         for (int c = 0; c < C; ++c) top_rows[(size_t)c * RS] = Nb[c];
     }
+    PINN_PHASE_ADD(PINN_PHASE_PROG, t_prog);
 #pragma unroll 1
     for (int l = Ln - 1; l >= 1; --l) {
+        PINN_PHASE_T0(t_rev);
         const DevLayer& L = P.layer[l];
         float* out_rows = units + (size_t)L.unit_base * C * RS;
         const DevLayer& B = P.layer[l - 1];                 // the layer below
@@ -1237,11 +1329,15 @@ PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weigh
             if (L.n_out == 1) bwd_layer<NF, NS, 1, false, GEN>(L, B.act, sw, out_rows, in_rows, RS, sink, in_rows, B.act, nullptr, nullptr, scr);
             else              bwd_layer<NF, NS, 4, false, GEN>(L, B.act, sw, out_rows, in_rows, RS, sink, in_rows, B.act, nullptr, nullptr, scr);
         }
+        PINN_PHASE_ADD(PINN_PHASE_REV + l, t_rev);
     }
     {
+        PINN_PHASE_T0(t_rev);
         const DevLayer& L = P.layer[0];
         float* out_rows = units + (size_t)L.unit_base * C * RS;
-        wgrad_input_layer<NF, NS>(L, out_rows, coords, RS, &P.dir_vec[0][0], sink);
+        if (L.n_in + 1 <= 4) wgrad_input_layer<NF, NS, 4>(L, out_rows, coords, RS, &P.dir_vec[0][0], sink);
+        else                 wgrad_input_layer<NF, NS, PINN_MAX_DIMS>(L, out_rows, coords, RS, &P.dir_vec[0][0], sink);
+        PINN_PHASE_ADD(PINN_PHASE_REV, t_rev);
     }
     return r;
 }

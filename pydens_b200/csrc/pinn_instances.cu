@@ -78,3 +78,16 @@ const bool entered = enter_all(std::make_integer_sequence<int, PINN_HI - PINN_LO
 
 }  // namespace
 }  // namespace pinn
+
+#if defined(PINN_PHASE_CLOCK)
+// Measurement builds only (tools/phase_clock.py compiles one unit with it): copy this unit's phase cycles
+// (PINN_PHASE_SLOTS counters) to `out`, and zero them when `reset`.
+extern "C" int pinn_phase_cycles_read(unsigned long long* out, int reset) {
+    if (cudaMemcpyFromSymbol(out, pinn_phase_cycles, sizeof(pinn_phase_cycles)) != cudaSuccess) return 1;
+    if (reset) {
+        static const unsigned long long zero[PINN_PHASE_SLOTS] = {};
+        if (cudaMemcpyToSymbol(pinn_phase_cycles, zero, sizeof(zero)) != cudaSuccess) return 1;
+    }
+    return 0;
+}
+#endif

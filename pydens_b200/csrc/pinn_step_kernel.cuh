@@ -462,15 +462,30 @@ __device__ __forceinline__ void step_body(const DevPlan& P, const StepArgs& a) {
 #pragma unroll
     for (int i = 0; i < PINN_MAX_VARS; ++i) part.vbar[i] = 0.0f;
 
+    // explicit batches: the coordinates of this warp's next tile are loaded into registers while the current tile runs
+    // (the batch pool is larger than L2, so each load would otherwise stall the warp for a trip to HBM)
+    float next_pt[PINN_MAX_DIMS];
+    auto load_tile = [&](long long tile) {
+        const long long pl = tile * 32 + lane;
+        const float* src = a.points + (size_t)(pl < a.n_points ? pl : a.n_points - 1) * P.total;
+#pragma unroll
+        for (int k = 0; k < PINN_MAX_DIMS; ++k)
+            if (k < P.total) next_pt[k] = __ldg(src + k);
+    };
     // tiles are dealt warp-slot-major (slot w of every CTA before slot w+1 of any): the last, partial round of tiles
     // spreads over all SMs instead of filling the first CTAs and leaving the others idle
-    for (long long tile = (long long)warp * gridDim.x + blockIdx.x; tile < n_tiles; tile += total_warps) {
+    const long long first_tile = (long long)warp * gridDim.x + blockIdx.x;
+    if (a.points && first_tile < n_tiles) load_tile(first_tile);
+    for (long long tile = first_tile; tile < n_tiles; tile += total_warps) {
+        PINN_PHASE_T0(t_load);
         const long long pl = tile * 32 + lane;
         const bool valid = pl < a.n_points;
         const long long pe = valid ? pl : a.n_points - 1;     // masked lanes replay the last point
         if (a.points) {
-            const float* src = a.points + (size_t)pe * P.total;
-            for (int k = 0; k < P.total; ++k) st[k * RS] = __ldg(src + k);
+#pragma unroll
+            for (int k = 0; k < PINN_MAX_DIMS; ++k)
+                if (k < P.total) st[k * RS] = next_pt[k];
+            if (tile + total_warps < n_tiles) load_tile(tile + total_warps);
         } else {
             const uint64_t gidx = a.point_offset + (uint64_t)pe;
             Philox4 b0 = philox_block(gidx, step, a.seed, 0u);
@@ -478,11 +493,13 @@ __device__ __forceinline__ void step_body(const DevPlan& P, const StepArgs& a) {
             if (P.total > 4) b1 = philox_block(gidx, step, a.seed, 1u);
             for (int k = 0; k < P.total; ++k) st[k * RS] = sample_column(P.cols[k], k, gidx, step, a.seed, b0, b1);
         }
+        PINN_PHASE_ADD(PINN_PHASE_LOAD, t_load);
         float r = point_step<NF, NS, JF, GEN, MULTI>(P, sw, a.params, st, RS, valid, a.inv_n, sink, part);
         if (a.residual && valid) a.residual[pl] = r;
     }
 
     // per-thread scalars -> accumulator
+    PINN_PHASE_T0(t_tail);
     {
         float v = warp_sum(part.loss);
         if (lane == 0) sink.add(P.n_params, v);
@@ -501,6 +518,7 @@ __device__ __forceinline__ void step_body(const DevPlan& P, const StepArgs& a) {
     // CTA partial -> global, then the last CTA folds all partials in block order
     cta_partial(a, wacc_all, n_out_floats, nwarps);
     finish_grid(a, n_out_floats);
+    PINN_PHASE_ADD(PINN_PHASE_TAIL, t_tail);
 }
 
 template <int NF, int NS, bool GMEM, int MAXT, int JF, bool GEN>
