@@ -124,7 +124,8 @@ typedef struct PinnColumn {
  *
  * Network (reference ConvBlockModel.forward model_torch.py:170-172, layouts 'fa…f'):
  *   n_layers linear layers, widths[0] = ndims + nparams, widths[n_layers] = k, the number of outputs: 1, or 2..4 for
- *   coupled systems (thread kernel, derivative order <= 2, nf <= 4; see Programs);
+ *   coupled systems (derivative order <= 2, nf <= 4; see Programs), which run on the thread kernel, or on the tile
+ *   kernel's 128-wide class when their 65-128-wide hidden layers do not fit the thread kernel's shared memory;
  *   act[l] is the activation applied AFTER linear layer l (0-based); act[n_layers-1] must
  *   be PINN_ACT_NONE.  skip_src[l] = s >= 0 adds the output of layer s (after ITS activation and skip)
  *   to the activated output of layer l (residual connections 'R … +').
@@ -418,7 +419,8 @@ typedef struct PinnPlanInfo {
     int32_t tensor_core;              /* 1: the tensor-core tile kernel for wide networks runs the step (3xTF32,
                                             hidden widths <= 64),
                                          2: its 128-wide class runs it (hidden widths up to 128; networks whose
-                                            weights the thread kernel cannot hold in shared memory),
+                                            weights the thread kernel cannot hold in shared memory, with 1 or
+                                            2..4 outputs),
                                          0: the thread-per-point FP32 kernel                 */
     int32_t small_batch_points;       /* largest batch the cluster (point, unit)-parallel loop kernel takes through
                                          pinn_multi_step (8 CTAs x 128 points), 0: the network does not fit it         */

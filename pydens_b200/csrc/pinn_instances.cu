@@ -12,10 +12,11 @@
 #define PINN_SMALL 6         // small_step_kernel, the tiny-batch cluster kernel
 #define PINN_WIDE128 7       // wide_step_kernel of the 128-wide class
 #define PINN_COUPLED 8       // coupled_step_kernel, networks of 2..4 outputs
+#define PINN_WIDE128_COUPLED 9   // wide128_coupled_step_kernel, networks of 2..4 outputs on the 128-wide class
 
 #if PINN_UNIT == PINN_HI_JET
 #include "pinn_hi_kernel.cuh"
-#elif PINN_UNIT == PINN_WIDE || PINN_UNIT == PINN_WIDE128
+#elif PINN_UNIT == PINN_WIDE || PINN_UNIT == PINN_WIDE128 || PINN_UNIT == PINN_WIDE128_COUPLED
 #include "pinn_wide_kernel.cuh"
 #elif PINN_UNIT == PINN_SMALL
 #include "pinn_small_kernel.cuh"
@@ -63,6 +64,8 @@ void enter() {
     CoupledSet& k = coupled_slot(NF, J);
     k.step[0] = coupled_step_kernel<NF, J, false, Cfg::MAXT>;
     k.step[1] = coupled_step_kernel<NF, J, true, Cfg::MAXT>;
+#elif PINN_UNIT == PINN_WIDE128_COUPLED
+    coupled_slot(NF, J).wide128 = wide::wide128_coupled_step_kernel<NF, J>;
 #else
 #error "PINN_UNIT names no kernel family"
 #endif

@@ -97,6 +97,10 @@ __global__ void __launch_bounds__(256, 1) coupled_forward_kernel(const __grid_co
 __global__ void __launch_bounds__(512, 1) wide::wide128_forward_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
     wide::wide_step<0, 0, 512, 128, true>(P, a);
 }
+// ... and of its coupled form: u_out [n, k]
+__global__ void __launch_bounds__(512, 1) wide::wide128_coupled_forward_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
+    wide::wide_step<0, 0, 512, 128, true, true>(P, a);
+}
 
 // Points the in-kernel sampler produces (for tests / replay).
 struct SampleCols { PinnColumn c[PINN_MAX_DIMS]; int total; };
@@ -150,10 +154,11 @@ static int fail(int code, const char* fmt, ...) {
 
 // The tensor-core tile kernel (pinn_wide_kernel.cuh) covers plain dense chains with polynomial-family activations
 // and hidden widths <= 128, in two width classes (<= 64 and 65..128); it pays off once the layers are wide enough to
-// be real GEMMs.  *max_width: the widest hidden layer.
+// be real GEMMs.  Networks of 2..4 outputs pass the same rules; only the 128-wide class has their (coupled) form.
+// *max_width: the widest hidden layer.
 static bool wide_eligible(const pinn::DevPlan& h, int* max_width) {
     if (h.n_layers < 2 || h.n_layers > pinn::wide::MAX_LAYERS) return false;
-    if (h.layer[h.n_layers - 1].n_out != 1) return false;           // networks of several outputs: thread kernel only
+    if (h.layer[h.n_layers - 1].n_out > 4) return false;
     int mw = 0;
     for (int l = 0; l < h.n_layers; ++l) {
         const pinn::DevLayer& L = h.layer[l];
@@ -179,7 +184,8 @@ struct PinnPlan {
     int wide_ctas;                           // CTAs the tile kernel runs on (<= sm_count)
     const KernelSet* ks;                     // the kernels of this plan's jet set
     StepKernelFn fn_smem, fn_gmem;           // the pair matching this plan (plain or general, or coupled_step_kernel)
-    bool coupled;                            // a network of 2..4 outputs: coupled_step_kernel / coupled_forward_kernel
+    bool coupled;                            // a network of 2..4 outputs: coupled_step_kernel / coupled_forward_kernel,
+                                             // or the coupled form of the 128-wide tile kernel
     int sm_count;
     int smem_optin;
     // step kernel launch config
@@ -330,17 +336,21 @@ static int place_wide_kernel(PinnPlan* p, int order, int thread_rc) {
     int mw = 0;
     const char* fk = getenv("PINN_FORCE_KERNEL");
     const bool eligible = order < 3 && wide_eligible(p->h, &mw);
-    const bool eligible128 = eligible && mw > 64 && p->ks->wide128;
+    // networks of 2..4 outputs: the coupled form of the 128-wide class only
+    const CoupledSet* cs = p->coupled ? coupled_kernels(p->h.nf, p->h.ns) : nullptr;
+    const StepKernelFn f128 = p->coupled ? (cs ? cs->wide128 : nullptr) : p->ks->wide128;
+    const bool eligible64 = eligible && !p->coupled;
+    const bool eligible128 = eligible && mw > 64 && f128;
     // the tile kernel wins from 64-wide layers with many jet channels on (H100 80GB HBM3 at 700 W, cfg5: 21.1 ms
     // vs 32.3 ms per step); for narrower networks the per (unit, channel) operand handling costs as much as the
     // FMA row it replaces, and the CUDA-core kernel keeps them.  Networks of 65-128 units the thread kernel holds
     // stay there: the 128-wide class takes only what the thread kernel refuses.
-    bool want = eligible && mw <= 64 && mw >= 48 && (1 + p->spec.nf + p->spec.ns) >= 5;
+    bool want = eligible64 && mw <= 64 && mw >= 48 && (1 + p->spec.nf + p->spec.ns) >= 5;
     int kw = 64;
     if (thread_rc != PINN_OK) { want = eligible128; kw = 128; }
     if (fk && !strcmp(fk, "thread")) want = false;
     if (fk && !strcmp(fk, "wide")) {
-        if (!eligible || mw > 64) return fail(PINN_E_UNSUPPORTED, "PINN_FORCE_KERNEL=wide: this network is outside what the tile kernel covers");
+        if (!eligible64 || mw > 64) return fail(PINN_E_UNSUPPORTED, "PINN_FORCE_KERNEL=wide: this network is outside what the tile kernel covers");
         want = true; kw = 64;
     }
     if (fk && !strcmp(fk, "wide128")) {
@@ -349,9 +359,10 @@ static int place_wide_kernel(PinnPlan* p, int order, int thread_rc) {
     }
     int wide_threads = 512;                     // four threads per point; PINN_WIDE_THREADS=256: two (experiments, 64-wide class)
     { const char* wt = getenv("PINN_WIDE_THREADS"); if (wt && atoi(wt) == 256 && kw == 64) wide_threads = 256; }
-    const StepKernelFn f = kw == 128 ? p->ks->wide128 : p->ks->wide[wide_threads == 256 ? 1 : 0];
+    const StepKernelFn f = kw == 128 ? f128 : p->ks->wide[wide_threads == 256 ? 1 : 0];
     if (!want || !f || (thread_rc != PINN_OK && kw != 128)) return thread_rc;
-    const int smem = kw == 128 ? wide::Tile<128>::SMEM_BYTES : wide::Tile<64>::SMEM_BYTES;
+    const int smem = kw == 128 ? (p->coupled ? wide::Tile<128, true>::SMEM_BYTES : wide::Tile<128>::SMEM_BYTES)
+                               : wide::Tile<64>::SMEM_BYTES;
     cudaError_t e = cudaFuncSetAttribute((const void*)f, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(wide, smem=%d): %s", smem, cudaGetErrorString(e));
     cudaFuncAttributes fa;
@@ -361,7 +372,8 @@ static int place_wide_kernel(PinnPlan* p, int order, int thread_rc) {
     p->wide = true; p->wide_kw = kw; p->gmem = true; p->threads = wide_threads; p->wacc_gmem = false;
     p->smem_bytes = smem; p->regs = fa.numRegs;
     if (thread_rc != PINN_OK) {                 // the forward kernel does not hold this network either
-        e = cudaFuncSetAttribute((const void*)wide::wide128_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        const void* ff = p->coupled ? (const void*)wide::wide128_coupled_forward_kernel : (const void*)wide::wide128_forward_kernel;
+        e = cudaFuncSetAttribute(ff, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
         if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(wide forward, smem=%d): %s", smem, cudaGetErrorString(e));
         p->fwd_wide = true; p->fwd_gmem = false;
     }
@@ -839,6 +851,8 @@ extern "C" int pinn_forward(const PinnPlan* p, const float* params, const float*
         w.params = params; w.points = points; w.n_points = n_points; w.out = u_out; w.ring_len = 1;
         const long long tiles = (n_points + wide::Tile<128>::T - 1) / wide::Tile<128>::T;
         const int grid = (int)(tiles < p->sm_count ? tiles : p->sm_count);
+        if (p->coupled)                        // u_out [n, k]
+            return launch_step(wide::wide128_coupled_forward_kernel, grid, 512, wide::Tile<128, true>::SMEM_BYTES, st, p->h, w);
         return launch_step(wide::wide128_forward_kernel, grid, 512, wide::Tile<128>::SMEM_BYTES, st, p->h, w);
     }
     FwdArgs a;

@@ -687,10 +687,12 @@ struct KernelSet {
     StepKernelFn wide128;                    // the tile kernel's class for hidden widths up to 128, 512 threads
 };
 
-// The step kernels of one jet set for networks of 2..4 outputs: coupled_step_kernel [GMEM].  Their own table, filled by
-// the 'coupled' build units; coupled_kernels(nf, ns) is nullptr outside 0 <= ns <= nf <= 4.
+// The step kernels of one jet set for networks of 2..4 outputs: coupled_step_kernel [GMEM], and the coupled form of the
+// 128-wide tile kernel.  Their own table, filled by the 'coupled' and 'wide128_coupled' build units;
+// coupled_kernels(nf, ns) is nullptr outside 0 <= ns <= nf <= 4.
 struct CoupledSet {
     StepKernelFn step[2];
+    StepKernelFn wide128;                    // wide128_coupled_step_kernel (pinn_wide_kernel.cuh), 512 threads
 };
 const CoupledSet* coupled_kernels(int nf, int ns);
 CoupledSet& coupled_slot(int nf, int ns);

@@ -28,10 +28,14 @@
 //     level); the adjoint of a level overwrites the dead slot of the level above.
 //   * wide128_forward_kernel is the forward-only form of the 128-wide class (pinn_forward): the value channel's
 //     forward sweep and the ansatz, no slab.
+//   * The 128-wide class has a coupled form (wide128_coupled_step_kernel / wide128_coupled_forward_kernel) for
+//     networks of 2..4 outputs, the same body with MULTI = true: the output GEMM's columns are the components, and
+//     the output layer's weight gradient is one small GEMM per jet channel against the components' adjoint seeds.
 //
 // Covered: dense chains 'fa…f' with tanh / sigmoid / identity hidden activations, 2 to 6 linear layers (MAX_LAYERS),
 // the jet sets NS <= NF <= 4, every ansatz / residual program / sampler the thread kernel covers; hidden widths <= 64
-// (tests/test_gpu_tile.py) or <= 128 with at least one above 64 (tests/test_gpu_tile128.py).  Everything else
+// (tests/test_gpu_tile.py) or <= 128 with at least one above 64 (tests/test_gpu_tile128.py); networks of 2..4
+// outputs on the 128-wide class only (tests/test_gpu_tile128_coupled.py).  Everything else
 // (residual layouts, sin/softplus/SiLU/GELU, wider layers, more layers, orders 3 / 4) stays on the thread kernels.
 #pragma once
 
@@ -49,7 +53,10 @@ __host__ __device__ constexpr int ilog2(int x) { return x <= 1 ? 0 : 1 + ilog2(x
 // The geometry of one width class KW (padded hidden width, 64 or 128).  The tile shrinks as the width grows,
 // T = 8192 / KW points, so that every [T][KW] operand, the slab block of a (level, channel) and the work-item count
 // of the data-gradient GEMM stay the same size; a thread still owns 16 hidden units at 512 threads.
-template <int KW_>
+// MULTI: the coupled form (networks of k = 2..4 outputs).  Its exchange area holds the k C adjoint seeds (k C <= 36)
+// beside the coordinates, its misc area k rows of output weights and one output-bias sum per component and warp; the
+// one-output map is unchanged.
+template <int KW_, bool MULTI = false>
 struct Tile {
     static constexpr int KW = KW_;
     static constexpr int T = TILE_FLOATS / KW;             // points per tile: 128 (KW = 64) or 64 (KW = 128)
@@ -66,14 +73,17 @@ struct Tile {
     static constexpr int S_A = S_W + KW * LDS * 4;         // A operand [T p][LDS]: jets (forward), delta (reverse)
     static constexpr int S_GB = S_A + T * LDS * 4;         // weight-gradient B operand: post-activation a_{h-1} [T p][LDS]
     static constexpr int S_D = S_GB + T * LDS * 4;         // GEMM result [T p][LDS]
-    static constexpr int S_X = S_D + T * LDS * 4;          // exchange area between the threads of a point [24][T]
-    static constexpr int S_XB = S_X + 24 * T * 4;          // small right-hand sides [16 rows][LXB]
+    static constexpr int KMAX = MULTI ? 4 : 1;             // network outputs
+    static constexpr int X_CRD = MULTI ? 36 : 16;          // exchange area: adjoint seeds in rows 0.., coordinates from X_CRD
+    static constexpr int X_ROWS = X_CRD + PINN_MAX_DIMS;
+    static constexpr int S_X = S_D + T * LDS * 4;          // exchange area between the threads of a point [X_ROWS][T]
+    static constexpr int S_XB = S_X + X_ROWS * T * 4;      // small right-hand sides [16 rows][LXB]
     static constexpr int S_WACC = S_XB + 16 * LXB * 4;     // hidden->hidden weight gradients (KW = 64 only)
     static constexpr int S_SMALL1 = S_WACC + (WACC_SMEM ? WACC_FLOATS * 4 : 0);  // level 1: first-layer W / b gradients [KW k][16]
     static constexpr int S_OUT = S_SMALL1 + KW * 16 * 4;   // output-layer weight gradient [KW k][8]
     static constexpr int S_SMALLH = S_OUT + KW * 8 * 4;    // level h >= 2: bias gradient of layer h-1 [4][KW j][8]
     static constexpr int S_MISC = S_SMALLH + (MAX_LAYERS - 2) * KW * 8 * 4;   // biases, first-layer weights, scalars
-    static constexpr int MISC_FLOATS = 24 * KW;
+    static constexpr int MISC_FLOATS = (MULTI ? 26 : 24) * KW;
     static constexpr int SMEM_BYTES = S_MISC + MISC_FLOATS * 4;
     static constexpr int ACC_FLOATS = (S_MISC - S_WACC) / 4;   // every shared-memory accumulator, zeroed once per launch
 
@@ -81,9 +91,10 @@ struct Tile {
     static constexpr int M_BIAS = 0;                           // [MAX_LAYERS][KW]
     static constexpr int M_W0 = M_BIAS + MAX_LAYERS * KW;      // first layer [KW][8]
     static constexpr int M_WD = M_W0 + KW * 8;                 // first layer applied to the direction vectors [6][KW]
-    static constexpr int M_WOUT = M_WD + PINN_MAX_DIRS * KW;   // output layer weights [KW]
-    static constexpr int M_SCAL = M_WOUT + KW;                 // per warp: loss, sbar, bout, vbar[4]  (8 floats each)
-    static constexpr int M_END = M_SCAL + 8 * (NT_MAX / 32);
+    static constexpr int M_WOUT = M_WD + PINN_MAX_DIRS * KW;   // output layer weights [KMAX j][KW]
+    static constexpr int M_SCAL = M_WOUT + KMAX * KW;          // per warp: loss, sbar, bout[KMAX], vbar[4]  (SCS floats each)
+    static constexpr int SCS = MULTI ? 16 : 8;
+    static constexpr int M_END = M_SCAL + SCS * (NT_MAX / 32);
 
     static_assert(KW == 64 || KW == 128, "width classes");
     static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one CTA");
@@ -257,9 +268,9 @@ __device__ __forceinline__ void gemm_wgrad(uint8_t* smem, float* acc_s, int mrow
 }
 // ACC[KW j x n] (row stride n) += GA^T . XB^T over the tile (XB: [16 rows][LXB]), n = 8 or 16.  The work items
 // (16 x 8 blocks) are dealt from the last warp down, so that they land beside the items of gemm_wgrad.
-template <int KW>
+template <int KW, bool MULTI = false>
 __device__ __forceinline__ void gemm_small(uint8_t* smem, float* acc_s, int n, int warp, int n_warps) {
-    using G = Tile<KW>;
+    using G = Tile<KW, MULTI>;
     constexpr int LDS = G::LDS, MB = KW / 16;
     const float* GA = reinterpret_cast<const float*>(smem + G::S_A);
     const float* XB = reinterpret_cast<const float*>(smem + G::S_XB);
@@ -291,10 +302,14 @@ __device__ __forceinline__ void gemm_small(uint8_t* smem, float* acc_s, int n, i
 // ---------------------------------------------------------------------------------------------------------------
 // The body of the kernels below.  KW: the width class (hidden widths <= 64 or <= 128).  FWD: the forward-only form
 // (pinn_forward), with NF = NS = 0: forward sweep of the value channel, ansatz, u of every point to a.out; no slab, no
-// reverse sweep.
-template <int NF, int NS, int NT, int KW, bool FWD>
+// reverse sweep.  MULTI: a network of k = P.layer[n_layers-1].n_out in 2..4 outputs (coupled systems), with the thread
+// kernel's conventions (point_step<…, MULTI>): the output GEMM's columns 0..k-1 are the k components' jets, the
+// ansatz is applied per component with the shared boundary factor and time gate, the residual program finds channel c
+// of component j in slot j*C + c and leaves its partial in slot eq_out[1] + j*C + c; the forward-only form writes
+// u [n, k] row-major.
+template <int NF, int NS, int NT, int KW, bool FWD, bool MULTI = false>
 __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
-    using G = Tile<KW>;
+    using G = Tile<KW, MULTI>;
     constexpr int T = G::T, LDS = G::LDS, LXB = G::LXB;
     constexpr int C = 1 + NF + NS;
     constexpr int NH = NT / T;               // threads per point: each owns KW / NH hidden units
@@ -307,6 +322,7 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
     const int tid = threadIdx.x, p = tid & (T - 1), kh = tid >> G::TSH, warp = tid >> 5, lane = tid & 31;
     const int warp_u = __shfl_sync(0xffffffffu, tid >> 5, 0);        // the same number, provably warp-uniform
     const int Ln = P.n_layers, H = Ln - 1;
+    const int K = MULTI ? P.layer[H].n_out : 1;                     // network outputs
     const int n_out_floats = P.n_params + 4;
     // hidden->hidden weight-gradient accumulators [4][KW][KW]: shared memory, or this CTA's area of the workspace
     float* const wacc_base = G::WACC_SMEM ? reinterpret_cast<float*>(smem + G::S_WACC)
@@ -335,7 +351,12 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
             if (k < L0.n_out) for (int q = 0; q < L0.n_in; ++q) sum = fmaf(__ldg(a.params + L0.w_off + k * L0.n_in + q), P.dir_vec[d][q], sum);
             misc[G::M_WD + d * KW + k] = sum;
         }
-        for (int k = tid; k < P.layer[H].n_in; k += NT) misc[G::M_WOUT + k] = __ldg(a.params + P.layer[H].w_off + k);
+        if constexpr (MULTI) {
+            for (int i = tid; i < K * P.layer[H].n_in; i += NT)
+                misc[G::M_WOUT + (i / P.layer[H].n_in) * KW + i % P.layer[H].n_in] = __ldg(a.params + P.layer[H].w_off + i);
+        } else {
+            for (int k = tid; k < P.layer[H].n_in; k += NT) misc[G::M_WOUT + k] = __ldg(a.params + P.layer[H].w_off + k);
+        }
     }
     __syncthreads();
 
@@ -353,7 +374,9 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
 
     const uint64_t step = a.step_ptr ? *a.step_ptr : a.step_val;
     const long long n_tiles = (a.n_points + T - 1) / T;
-    float acc_loss = 0.0f, acc_sbar = 0.0f, acc_bout = 0.0f, acc_vbar[PINN_MAX_VARS];
+    float acc_loss = 0.0f, acc_sbar = 0.0f, acc_bout[G::KMAX], acc_vbar[PINN_MAX_VARS];
+#pragma unroll
+    for (int j = 0; j < G::KMAX; ++j) acc_bout[j] = 0.0f;
 #pragma unroll
     for (int i = 0; i < PINN_MAX_VARS; ++i) acc_vbar[i] = 0.0f;
 
@@ -428,9 +451,9 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
         // level 1: the first linear layer acts on (x, direction vectors, 0) — per thread, no GEMM; only the
         // activations are stored
         float a0h[QN][8];                                    // activations of the current level, this thread's units
-        if (kh == 0) {                                       // the coordinates wait in the exchange area (rows 16..23)
+        if (kh == 0) {                                       // the coordinates wait in the exchange area (rows X_CRD..)
 #pragma unroll
-            for (int k = 0; k < PINN_MAX_DIMS; ++k) Xbuf[(16 + k) * T + p] = x[k];
+            for (int k = 0; k < PINN_MAX_DIMS; ++k) Xbuf[(G::X_CRD + k) * T + p] = x[k];
         }
         {
             const ActC kc = make_actc(P.layer[0].act);
@@ -474,6 +497,13 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
                         }
                         if constexpr (!FWD) st8<T>(row(h + 1, c), n0, z);
                     }
+                } else if constexpr (MULTI) {
+                    // columns 0..k-1: channel c of the k components, parked in the exchange area (row j*C + c)
+                    // until the ansatz reads them
+                    if (kh == 0)
+                        for (int j = 0; j < K; ++j)
+                            Xbuf[(j * C + c) * T + p] = reinterpret_cast<const float*>(smem + G::S_D)[p * LDS + j] +
+                                                        (c == 0 ? misc[G::M_BIAS + H * KW + j] : 0.0f);
                 } else {
                     N[c] = reinterpret_cast<const float*>(smem + G::S_D)[p * LDS] + (c == 0 ? misc[G::M_BIAS + H * KW] : 0.0f);
                 }
@@ -514,7 +544,7 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
             float* coords = st;
             float* scr = st + (size_t)PINN_MAX_DIMS * RS;
 #pragma unroll
-            for (int k = 0; k < PINN_MAX_DIMS; ++k) coords[(size_t)k * RS] = Xbuf[(16 + k) * T + p];
+            for (int k = 0; k < PINN_MAX_DIMS; ++k) coords[(size_t)k * RS] = Xbuf[(G::X_CRD + k) * T + p];
             float icj[C];
 #pragma unroll
             for (int c = 0; c < C; ++c) icj[c] = 0.0f;
@@ -526,49 +556,127 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
             const float log_scale = __ldg(a.params + P.log_scale_off);
             AnsatzState<NF, NS> as;
             float u[C];
-            ansatz_forward<NF, NS, true>(P, coords, RS, log_scale, N, icj, as, u);
-            if constexpr (FWD) {
-                if (valid) a.out[pl] = u[0];
-            } else {
+            if constexpr (MULTI) {
+                // one component at a time; its jets wait in the exchange area, where its adjoint seed replaces them
+                auto load_N = [&](int j) {
 #pragma unroll
-                for (int c = 0; c < C; ++c) scr[(size_t)c * RS] = u[c];
-                eval_prog(P.eq, P.n_eq, scr, RS, coords, a.params, P.var_off);
-                const float r = scr[(size_t)P.eq_out[0] * RS];
-                const float rb = valid ? 2.0f * r * a.inv_n : 0.0f;
-                if (valid) acc_loss = fmaf(r * a.inv_n, r, acc_loss);
-                if (a.residual && valid) a.residual[pl] = r;
-                float ub[C];
+                    for (int c = 0; c < C; ++c) N[c] = Xbuf[(j * C + c) * T + p];
+                };
+#pragma unroll 1
+                for (int j = 0; j < K; ++j) {
+                    load_N(j);
+                    ansatz_forward<NF, NS, true>(P, coords, RS, log_scale, N, icj, as, u);
+                    if constexpr (FWD) {
+                        if (valid) a.out[(size_t)pl * K + j] = u[0];
+                    } else {
 #pragma unroll
-                for (int c = 0; c < C; ++c) ub[c] = rb * scr[(size_t)P.eq_out[1 + c] * RS];
-#pragma unroll
-                for (int i = 0; i < PINN_MAX_VARS; ++i)
-                    if (i < P.n_vars) acc_vbar[i] = fmaf(rb, scr[(size_t)P.eq_out[1 + C + i] * RS], acc_vbar[i]);
-                if (P.ic_has_vars) {
-#pragma unroll
-                    for (int i = 0; i < PINN_MAX_VARS; ++i) {
-                        if (i < P.n_vars) {
-#pragma unroll
-                            for (int c = 0; c < C; ++c)
-                                acc_vbar[i] = fmaf(ub[c], scr[(size_t)P.ic_out[C * (1 + i) + c] * RS], acc_vbar[i]);
-                        }
+                        for (int c = 0; c < C; ++c) scr[(size_t)(j * C + c) * RS] = u[c];
                     }
                 }
-                acc_sbar += ansatz_adjoint<NF, NS>(P, as, ub, Nb);
-                acc_bout += Nb[0];
-                // the adjoint seed of the point goes to the exchange area (rows 0..C-1): every thread of the point reads
-                // it from there when it needs it, instead of carrying C registers through the reverse sweep
+                if constexpr (!FWD) {
+                    eval_prog(P.eq, P.n_eq, scr, RS, coords, a.params, P.var_off);
+                    const float r = scr[(size_t)P.eq_out[0] * RS];
+                    const float rb = valid ? 2.0f * r * a.inv_n : 0.0f;
+                    if (valid) acc_loss = fmaf(r * a.inv_n, r, acc_loss);
+                    if (a.residual && valid) a.residual[pl] = r;
 #pragma unroll
-                for (int c = 0; c < C; ++c) Xbuf[c * T + p] = Nb[c];
+                    for (int i = 0; i < PINN_MAX_VARS; ++i)
+                        if (i < P.n_vars) acc_vbar[i] = fmaf(rb, scr[(size_t)P.eq_out[1 + C + i] * RS], acc_vbar[i]);
+#pragma unroll 1
+                    for (int j = 0; j < K; ++j) {
+                        float ub[C];
+#pragma unroll
+                        for (int c = 0; c < C; ++c) ub[c] = rb * scr[(size_t)(P.eq_out[1] + j * C + c) * RS];
+                        if (P.ic_has_vars) {
+#pragma unroll
+                            for (int i = 0; i < PINN_MAX_VARS; ++i) {
+                                if (i < P.n_vars) {
+#pragma unroll
+                                    for (int c = 0; c < C; ++c)
+                                        acc_vbar[i] = fmaf(ub[c], scr[(size_t)P.ic_out[C * (1 + i) + c] * RS], acc_vbar[i]);
+                                }
+                            }
+                        }
+                        load_N(j);
+                        ansatz_forward<NF, NS, true>(P, coords, RS, log_scale, N, icj, as, u);   // component j's state again
+                        acc_sbar += ansatz_adjoint<NF, NS>(P, as, ub, Nb);
+#pragma unroll
+                        for (int jj = 0; jj < G::KMAX; ++jj)
+                            if (jj == j) acc_bout[jj] += Nb[0];
+#pragma unroll
+                        for (int c = 0; c < C; ++c) Xbuf[(j * C + c) * T + p] = Nb[c];
+                    }
+                }
+            } else {
+                ansatz_forward<NF, NS, true>(P, coords, RS, log_scale, N, icj, as, u);
+                if constexpr (FWD) {
+                    if (valid) a.out[pl] = u[0];
+                } else {
+#pragma unroll
+                    for (int c = 0; c < C; ++c) scr[(size_t)c * RS] = u[c];
+                    eval_prog(P.eq, P.n_eq, scr, RS, coords, a.params, P.var_off);
+                    const float r = scr[(size_t)P.eq_out[0] * RS];
+                    const float rb = valid ? 2.0f * r * a.inv_n : 0.0f;
+                    if (valid) acc_loss = fmaf(r * a.inv_n, r, acc_loss);
+                    if (a.residual && valid) a.residual[pl] = r;
+                    float ub[C];
+#pragma unroll
+                    for (int c = 0; c < C; ++c) ub[c] = rb * scr[(size_t)P.eq_out[1 + c] * RS];
+#pragma unroll
+                    for (int i = 0; i < PINN_MAX_VARS; ++i)
+                        if (i < P.n_vars) acc_vbar[i] = fmaf(rb, scr[(size_t)P.eq_out[1 + C + i] * RS], acc_vbar[i]);
+                    if (P.ic_has_vars) {
+#pragma unroll
+                        for (int i = 0; i < PINN_MAX_VARS; ++i) {
+                            if (i < P.n_vars) {
+#pragma unroll
+                                for (int c = 0; c < C; ++c)
+                                    acc_vbar[i] = fmaf(ub[c], scr[(size_t)P.ic_out[C * (1 + i) + c] * RS], acc_vbar[i]);
+                            }
+                        }
+                    }
+                    acc_sbar += ansatz_adjoint<NF, NS>(P, as, ub, Nb);
+                    acc_bout[0] += Nb[0];
+                    // the adjoint seed of the point goes to the exchange area (rows 0..C-1): every thread of the point
+                    // reads it from there when it needs it, instead of carrying C registers through the reverse sweep
+#pragma unroll
+                    for (int c = 0; c < C; ++c) Xbuf[c * T + p] = Nb[c];
+                }
             }
         }
         if constexpr (FWD) continue;                         // the forward-only form ends its tile here
-        auto nb_of = [&](int c) { return Xbuf[c * T + p]; };
+        auto nb_of = [&](int c) { return Xbuf[c * T + p]; };  // adjoint seed row (MULTI: row j*C + c, component j)
         __syncthreads();
 
         // =========================== reverse ===========================
         // the output layer (one unit): its weight gradient  Wbar_out[k] = sum_p sum_c Nb[c] a_{H,c}[k]  is ONE small
-        // GEMM of the per-point sums against a column of ones; abar_{H,c}[k] = w_out[k] Nb[c] needs no GEMM at all
-        {
+        // GEMM of the per-point sums against a column of ones; abar_{H,c}[k] = w_out[k] Nb[c] needs no GEMM at all.
+        // MULTI (k units): Wbar_out[j][k] = sum_c sum_p Nb[j][c] a_{H,c}[k] is one small GEMM per channel c, with
+        // A = a_{H,c} and right-hand-side row j = Nb[j][c], into column j of the accumulator
+        if constexpr (MULTI) {
+            const ActC kc = make_actc(P.layer[H - 1].act);
+            auto out_gemm = [&](int c) {
+                if (kh == 0)
+                    for (int j = 0; j < K; ++j) xb[j * LXB + p] = nb_of(j * C + c);
+                sync_issue([&](int w) { gemm_small<KW, MULTI>(smem, reinterpret_cast<float*>(smem + G::S_OUT), 8, w, NT / 32); });
+            };
+            for (int g = 0; g <= NF; ++g) {
+                const int cy = group_y(g);
+                float stash[QN][8];
+#pragma unroll
+                for (int q = 0; q < QN; ++q) {
+                    float ax[8];
+                    post_group(H, g, kbeg + q * 8, kc, a0h[q], ax, stash[q]);
+                    put_A(kbeg + q * 8, ax);
+                }
+                out_gemm(group_x(g));
+                if (cy >= 0) {
+#pragma unroll
+                    for (int q = 0; q < QN; ++q) put_A(kbeg + q * 8, stash[q]);
+                    out_gemm(cy);
+                }
+            }
+        } else {
             const ActC kc = make_actc(P.layer[H - 1].act);
 #pragma unroll
             for (int q = 0; q < QN; ++q) {
@@ -593,7 +701,7 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
                 put_A(k0, t);
             }
             if (kh == 0) xb[p] = 1.0f;
-            sync_issue([&](int w) { gemm_small<KW>(smem, reinterpret_cast<float*>(smem + G::S_OUT), 8, w, NT / 32); });
+            sync_issue([&](int w) { gemm_small<KW, MULTI>(smem, reinterpret_cast<float*>(smem + G::S_OUT), 8, w, NT / 32); });
         }
         // rounds H..1: adjoint through the activation of level h, then (h >= 2) through the linear layer below it
         for (int h = H; h >= 1; --h) {
@@ -616,7 +724,16 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
                 for (int i = 0; i < 8; ++i) R[q][i] = 0.0f;
             // adjoint of the post-activation jet channel c of level h, units k0..k0+7
             auto ld_ab = [&](int c, int k0, float (&v)[8]) {
-                if (h == H) {
+                if (h == H && MULTI) {                       // sum_j W_out[j][k] Nb[j][c]
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) v[i] = 0.0f;
+#pragma unroll 1
+                    for (int j = 0; j < K; ++j) {
+                        const float nb = nb_of(j * C + c);
+#pragma unroll
+                        for (int i = 0; i < 8; ++i) v[i] = fmaf(misc[G::M_WOUT + j * KW + k0 + i], nb, v[i]);
+                    }
+                } else if (h == H) {
                     const float nb = nb_of(c);
 #pragma unroll
                     for (int i = 0; i < 8; ++i) v[i] = misc[G::M_WOUT + k0 + i] * nb;
@@ -632,7 +749,7 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
                     if (h == 1) {
 #pragma unroll
                         for (int i = 0; i < PINN_MAX_DIMS; ++i)
-                            if (i < P.total) xb[(1 + i) * LXB + p] = (c == 0) ? Xbuf[(16 + i) * T + p] : ((c <= NF) ? P.dir_vec[d][i] : 0.0f);
+                            if (i < P.total) xb[(1 + i) * LXB + p] = (c == 0) ? Xbuf[(G::X_CRD + i) * T + p] : ((c <= NF) ? P.dir_vec[d][i] : 0.0f);
                     }
                 }
                 if (h >= 2) {
@@ -642,7 +759,7 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
                     sync_issue([&](int w) {
                         gemm_rows<KW>(smem, kp, np, w, NT / 32);
                         gemm_wgrad<KW>(smem, wacc_base + (h - 2) * KW * KW, L.n_out, L.n_in, w, NT / 32);
-                        if (c == 0) gemm_small<KW>(smem, reinterpret_cast<float*>(smem + G::S_SMALLH) + (h - 2) * KW * 8, 8, w, NT / 32);
+                        if (c == 0) gemm_small<KW, MULTI>(smem, reinterpret_cast<float*>(smem + G::S_SMALLH) + (h - 2) * KW * 8, 8, w, NT / 32);
                     });
                     float* dst = row(h, c);                  // abar_{h-1,c} takes the dead slot of (h, c)
 #pragma unroll
@@ -657,7 +774,7 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
                         st8<T>(dst, n0, z);
                     }
                 } else {                                     // level 1: only the first layer's own gradients
-                    sync_issue([&](int w) { gemm_small<KW>(smem, reinterpret_cast<float*>(smem + G::S_SMALL1), 16, w, NT / 32); });
+                    sync_issue([&](int w) { gemm_small<KW, MULTI>(smem, reinterpret_cast<float*>(smem + G::S_SMALL1), 16, w, NT / 32); });
                 }
             };
             auto put_ops = [&](int k0, const float (&delta)[8], const float (&below)[8]) {
@@ -738,17 +855,20 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
     for (int i = tid; i < n_out_floats; i += NT) mine[i] = 0.0f;
     {
         // per-warp slots, summed in warp order below: no float atomics, bit-reproducible run to run
-        float* slot = misc + G::M_SCAL + 8 * warp;
+        float* slot = misc + G::M_SCAL + G::SCS * warp;
         float v = warp_sum(acc_loss);
         if (lane == 0) slot[0] = v;
         v = warp_sum(acc_sbar);
         if (lane == 0) slot[1] = v;
-        v = warp_sum(acc_bout);
-        if (lane == 0) slot[2] = v;
+#pragma unroll
+        for (int j = 0; j < G::KMAX; ++j) {
+            v = warp_sum(acc_bout[j]);
+            if (lane == 0) slot[2 + j] = v;
+        }
 #pragma unroll
         for (int i = 0; i < PINN_MAX_VARS; ++i) {
             v = warp_sum(acc_vbar[i]);
-            if (lane == 0) slot[3 + i] = v;
+            if (lane == 0) slot[2 + G::KMAX + i] = v;
         }
     }
     __syncthreads();
@@ -769,20 +889,25 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
         }
         const float* outw = reinterpret_cast<const float*>(smem + G::S_OUT);
         const DevLayer& LO = P.layer[H];
-        for (int j = tid; j < LO.n_in; j += NT) mine[LO.w_off + j] = outw[j * 8];
+        if constexpr (MULTI) {                              // W_out[j][m]: row m, column j of the accumulator
+            for (int i = tid; i < K * LO.n_in; i += NT) mine[LO.w_off + i] = outw[(i % LO.n_in) * 8 + i / LO.n_in];
+        } else {
+            for (int j = tid; j < LO.n_in; j += NT) mine[LO.w_off + j] = outw[j * 8];
+        }
     }
     if (tid == 0) {
-        float sc[3 + PINN_MAX_VARS];
+        constexpr int NSC = 2 + G::KMAX + PINN_MAX_VARS;
+        float sc[NSC];
 #pragma unroll
-        for (int i = 0; i < 3 + PINN_MAX_VARS; ++i) {
+        for (int i = 0; i < NSC; ++i) {
             float t = 0.0f;
-            for (int w = 0; w < NT / 32; ++w) t += misc[G::M_SCAL + 8 * w + i];
+            for (int w = 0; w < NT / 32; ++w) t += misc[G::M_SCAL + G::SCS * w + i];
             sc[i] = t;
         }
         mine[P.n_params] = sc[0];
         mine[P.log_scale_off] = sc[1];
-        mine[P.layer[H].b_off] = sc[2];
-        for (int i = 0; i < P.n_vars; ++i) mine[P.var_off[i]] = sc[3 + i];
+        for (int j = 0; j < K; ++j) mine[P.layer[H].b_off + j] = sc[2 + j];
+        for (int i = 0; i < P.n_vars; ++i) mine[P.var_off[i]] = sc[2 + G::KMAX + i];
     }
     __syncthreads();
     finish_grid(a, n_out_floats);
@@ -798,8 +923,14 @@ template <int NF, int NS>
 __global__ void __launch_bounds__(512, 1) wide128_step_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
     wide_step<NF, NS, 512, 128, false>(P, a);
 }
-// pinn_forward of the networks only the 128-wide class holds: u of every point to a.out
+// the coupled form (networks of 2..4 outputs) of the 128-wide class
+template <int NF, int NS>
+__global__ void __launch_bounds__(512, 1) wide128_coupled_step_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
+    wide_step<NF, NS, 512, 128, false, true>(P, a);
+}
+// pinn_forward of the networks only the 128-wide class holds: u of every point to a.out (coupled: [n, k] row-major)
 __global__ void __launch_bounds__(512, 1) wide128_forward_kernel(const __grid_constant__ DevPlan P, const StepArgs a);
+__global__ void __launch_bounds__(512, 1) wide128_coupled_forward_kernel(const __grid_constant__ DevPlan P, const StepArgs a);
 
 }  // namespace wide
 }  // namespace pinn

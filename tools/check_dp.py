@@ -41,10 +41,13 @@ def main():
         import problems as P
         import problems_wide as PW         # ... or a 128-wide network (poisson_wide128)
         import problems_coupled as PC      # ... or a network of several outputs (navier_stokes2d)
+        import problems_wide_coupled as PWC    # ... or both (navier_stokes2d_wide)
         if problem in PW.PROBLEMS:
             P = PW
         elif problem in PC.PROBLEMS:
             P = PC
+        elif problem in PWC.PROBLEMS:
+            P = PWC
         cfg = P.PROBLEMS[problem]
         solver = Solver(P.bind(problem, D, lambda n, init: V(n, data=torch.Tensor([init]))), ndims=cfg['ndims'],
                         nparams=cfg['nparams'], initial_condition=cfg['ic'], boundary_condition=cfg['bc'],
