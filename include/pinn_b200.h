@@ -364,13 +364,38 @@ int pinn_step_adam(const PinnPlan* plan, const PinnComm* comm_or_null, float* pa
  *   step_counter                  device step number: Philox counter word and ring index, as in pinn_step; += k_steps
  *   losses_ring[(step) % ring_len] receives the loss of every step.
  * pinn_multi_step_max_points: largest batch the kernel takes (0: this network does not fit the kernel).
+ *
+ * pinn_multi_step_terms: the same with constraint terms (reference :451-457, `loss_terms=['equation', 'constraint_0']`).
+ * One optimizer step is the gradient of  point_weight * sum_batch r^2  +  sum_k term_k.point_weight * sum_{its points} r_k^2,
+ * and the logged loss is that sum.  point_weight is 1 / n_points for a mean criterion, 1 for reduction='sum'.
+ * A term is a constraint plan (pinn_plan_create on a spec with no derivative directions whose residual program is the
+ * constraint, evaluated on u at fixed points) with the same layer table, n_params and log_scale_off as `plan`, the same
+ * ansatz, and variables among the plan's.  Its points are read from HOST memory during the call and travel to the
+ * kernel by value, with the residual program: the call allocates nothing and stays stream-ordered and capturable.
+ * They do not consume sampler counters: an in-kernel batch is the one pinn_sample gives.  At most PINN_MAX_TERMS terms
+ * and PINN_MAX_TERM_POINTS points in all; n_points + the term points <= pinn_multi_step_max_points.  A term plan that
+ * does not match: PINN_E_INVALID.  pinn_multi_step is this call with point_weight = 1 / n_points and no terms.
  */
+#define PINN_MAX_TERMS        4
+#define PINN_MAX_TERM_POINTS 32
+typedef struct PinnTerm {
+    const PinnPlan* plan;      /* the constraint's plan */
+    int32_t n_points;          /* 1 .. PINN_MAX_TERM_POINTS */
+    float point_weight;        /* 1 / n_points (mean criterion) or 1 (reduction='sum') */
+    const float* points;       /* HOST [n_points, ndims+nparams] row-major fp32 */
+} PinnTerm;
 int pinn_multi_step_max_points(const PinnPlan* plan);
 int pinn_multi_step(const PinnPlan* plan, float* params, float* exp_avg, float* exp_avg_sq, const float* mask,
                     float* step_tensors, int n_step_tensors, const float* points, const PinnColumn* cols,
                     uint64_t seed, uint64_t* step_counter, int64_t n_points, int k_steps,
                     float lr, float beta1, float beta2, float eps, float weight_decay, float opt_step0,
                     float* losses_ring, int64_t ring_len, void* stream);
+int pinn_multi_step_terms(const PinnPlan* plan, float* params, float* exp_avg, float* exp_avg_sq, const float* mask,
+                          float* step_tensors, int n_step_tensors, const float* points, const PinnColumn* cols,
+                          uint64_t seed, uint64_t* step_counter, int64_t n_points, int k_steps,
+                          float lr, float beta1, float beta2, float eps, float weight_decay, float opt_step0,
+                          float* losses_ring, int64_t ring_len, float point_weight, int n_terms,
+                          const PinnTerm* terms, void* stream);
 
 /* Forward only: u = ansatz(net(x)) for explicit points — the work of Solver.predict
  * (model_torch.py:466-487) and of the `_forward` closure handed to constraints (:451-454).

@@ -118,6 +118,26 @@ struct alignas(16) DevPlan {
     PinnInstr ic[PINN_MAX_PROG];
 };
 
+// A constraint term of the persistent multi-step kernels (pinn_multi_step_terms): its residual program runs on u (the
+// value channel of the equation's ansatz) at fixed points.  Its slots are the constraint plan's: slot 0 holds u,
+// eq_out = [r, dr/du, dr/dV_i ..], and PINN_OP_VAR operands index ITS variable list (var_off: flat offsets);
+// var_map[i] is the equation variable with the same offset, whose partial it adds to.
+struct DevTerm {
+    int n_eq;
+    float weight;                       // the term's point weight: 1 / n (mean) or 1 (sum)
+    int var_off[PINN_MAX_VARS];
+    int var_map[PINN_MAX_VARS];
+    int n_vars;
+    int eq_out[2 + PINN_MAX_VARS];
+    PinnInstr eq[PINN_MAX_PROG];
+};
+struct DevTerms {
+    int n_terms, n_points;              // n_points: over all terms; term t owns points first[t] .. first[t+1]-1
+    int first[PINN_MAX_TERMS + 1];
+    float x[PINN_MAX_TERM_POINTS][PINN_MAX_DIMS];
+    DevTerm t[PINN_MAX_TERMS];
+};
+
 // ----------------------------------------------------------------------------------------------
 // Philox4x32-10 (Salmon et al., SC'11) — counter-based RNG for in-kernel collocation sampling.
 // Restated bit-exactly in oracle/philox.py.
@@ -1207,15 +1227,52 @@ PINN_HD void ic_var_partials(const DevPlan& P, const float* __restrict__ scr, in
     }
 }
 
+// A constraint term's point (DevTerm): the initial condition's d(ic)/dV_i of the value channel, read BEFORE the term's
+// program runs — that program's slots are the constraint plan's and may cover the equation plan's ic_out slots.
+template <int NF, int NS>
+PINN_HD void term_ic_partials(const DevPlan& P, const float* __restrict__ scr, int RS, float (&icv)[PINN_MAX_VARS]) {
+    constexpr int C = 1 + NF + NS;
+#pragma unroll
+    for (int i = 0; i < PINN_MAX_VARS; ++i)
+        icv[i] = (P.ic_has_vars && i < P.n_vars) ? scr[(size_t)P.ic_out[C * (1 + i)] * RS] : 0.0f;
+}
+// ... and, after it ran (rb = 2 r weight), the adjoint seeds of the jet — the value channel only — and the partials of the
+// equation's variables: dr/dV of the term's variables that share their offset, plus the initial condition's share.
+template <int NF, int NS>
+PINN_HD void term_seeds(const DevPlan& P, const DevTerm& T, const float* __restrict__ scr, int RS, float rb,
+                        const float (&icv)[PINN_MAX_VARS], float (&ub)[1 + NF + NS], PointPartials<NF, NS>& part) {
+    constexpr int C = 1 + NF + NS;
+    ub[0] = rb * scr[(size_t)T.eq_out[1] * RS];
+#pragma unroll
+    for (int c = 1; c < C; ++c) ub[c] = 0.0f;
+#pragma unroll
+    for (int j = 0; j < PINN_MAX_VARS; ++j) {
+        if (j < P.n_vars) {
+            for (int i = 0; i < T.n_vars; ++i)
+                if (T.var_map[i] == j) part.vbar[j] = fmaf(rb, scr[(size_t)T.eq_out[2 + i] * RS], part.vbar[j]);
+            if (P.ic_has_vars) part.vbar[j] = fmaf(ub[0], icv[j], part.vbar[j]);
+        }
+    }
+}
+// The term that owns term point i (DevTerms::first is ascending).
+PINN_HD int term_of(const DevTerms& T, int i) {
+    int t = 0;
+    for (int k = 1; k < T.n_terms; ++k) if (i >= T.first[k]) t = k;
+    return t;
+}
+
 // MULTI: a network of k = P.layer[n_layers-1].n_out in 2..4 outputs (coupled systems).  The k output jets live in the
 // output layer's storage rows (unit j, channel c), never in registers; the ansatz is applied to every component with
 // the shared boundary factor and time gate; the residual program finds channel c of component j in slot j*C + c and
 // leaves dr/d(that channel) in slot eq_out[1] + j*C + c.
-template <int NF, int NS, int JF, bool GEN = true, bool MULTI = false>
+// TERMS (one output): a point of a constraint term when `term` is set — the same forward jets, its own residual program
+// on the value channel, weight term->weight, zero adjoint seeds on the derivative channels (term_seeds).
+template <int NF, int NS, int JF, bool GEN = true, bool MULTI = false, bool TERMS = false>
 PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weights */,
                          const float* __restrict__ pvals /* flat params (for log_scale, V) */,
                          float* __restrict__ st, int RS, bool valid, float inv_n,
-                         const GradSink& sink, PointPartials<NF, NS>& part) {
+                         const GradSink& sink, PointPartials<NF, NS>& part, const DevTerm* term = nullptr) {
+    static_assert(!(TERMS && MULTI), "constraint terms: networks of one output");
     constexpr int C = 1 + NF + NS;
     const int Ln = P.n_layers;
     float* coords = st;
@@ -1271,11 +1328,27 @@ PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weigh
 #pragma unroll
         for (int c = 0; c < C; ++c) scr[(size_t)c * RS] = u[c];
     }
-    eval_prog(P.eq, P.n_eq, scr, RS, coords, pvals, P.var_off);
-    float r = scr[(size_t)P.eq_out[0] * RS];
+    float icv[PINN_MAX_VARS];
+    float r;
+    if (TERMS && term) {
+        term_ic_partials<NF, NS>(P, scr, RS, icv);
+        eval_prog(term->eq, term->n_eq, scr, RS, coords, pvals, term->var_off);
+        r = scr[(size_t)term->eq_out[0] * RS];
+        inv_n = term->weight;
+    } else {
+        eval_prog(P.eq, P.n_eq, scr, RS, coords, pvals, P.var_off);
+        r = scr[(size_t)P.eq_out[0] * RS];
+    }
     float rb = valid ? 2.0f * r * inv_n : 0.0f;
     if (valid) part.loss = fmaf(r * inv_n, r, part.loss);
-    if constexpr (MULTI) {
+    if (TERMS && term) {
+        float ub[C];
+        term_seeds<NF, NS>(P, *term, scr, RS, rb, icv, ub, part);
+        float Nb[C];
+        part.sbar += ansatz_adjoint<NF, NS>(P, as, ub, Nb);
+#pragma unroll
+        for (int c = 0; c < C; ++c) top_rows[(size_t)c * RS] = Nb[c];
+    } else if constexpr (MULTI) {
 #pragma unroll
         for (int i = 0; i < PINN_MAX_VARS; ++i)
             if (i < P.n_vars) part.vbar[i] = fmaf(rb, scr[(size_t)P.eq_out[1 + C + i] * RS], part.vbar[i]);

@@ -181,6 +181,7 @@ struct PinnPlan {
     int multi_threads, multi_smem;
     MultiKernelFn fn_small;                  // tiny-batch (<= 128 points) variant, or nullptr
     int small_smem;
+    int multi_budget, small_budget;          // dynamic shared memory the two can take (constraint programs with more slots)
     int wide_ctas;                           // CTAs the tile kernel runs on (<= sm_count)
     const KernelSet* ks;                     // the kernels of this plan's jet set
     StepKernelFn fn_smem, fn_gmem;           // the pair matching this plan (plain or general, or coupled_step_kernel)
@@ -289,21 +290,26 @@ static int place_forward_kernel(PinnPlan* p) {
 
 // Persistent multi-step kernel (small batches): per-point state + parameters + Adam moments in shared memory.  Left
 // out when the jet set has none or the network does not fit.
+// Dynamic shared memory of multi_step_kernel at `nw` warps and `rows` per-point rows.
+static int multi_smem_bytes(const DevPlan& h, int nw, int rows) {
+    const int n_out_floats = h.n_params + 4;
+    const int extra = 3 * align4(h.n_params) + align4(n_out_floats);
+    return (smem_layout(h.weights_floats, n_out_floats, nw, storage_floats(h, rows, nw)).total_f + extra) * 4;
+}
+
 static void place_multi_kernel(PinnPlan* p) {
-    p->fn_multi = nullptr; p->multi_threads = 0; p->multi_smem = 0;
+    p->fn_multi = nullptr; p->multi_threads = 0; p->multi_smem = 0; p->multi_budget = 0;
     const MultiKernelFn f = p->ks->multi;
     if (!f) return;
     cudaFuncAttributes fm;
     if (cudaFuncGetAttributes(&fm, (const void*)f) == cudaSuccess) {
         const DevPlan& h = p->h;
-        const int n_out_floats = h.n_params + 4;
-        const int extra = 3 * align4(h.n_params) + align4(n_out_floats);
         const int mbudget = p->smem_optin - (int)fm.sharedSizeBytes - 64;
         for (int nw = max_warps(fm, p->ks->maxt); nw >= 1 && !p->fn_multi; --nw) {
-            SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, nw, storage_floats(h, h.rows_total, nw));
-            if ((SL.total_f + extra) * 4 <= mbudget) {
+            const int bytes = multi_smem_bytes(h, nw, h.rows_total);
+            if (bytes <= mbudget) {
                 p->fn_multi = f; p->multi_threads = nw * 32;
-                p->multi_smem = (SL.total_f + extra) * 4;
+                p->multi_smem = bytes; p->multi_budget = mbudget;
             }
         }
         if (p->fn_multi && allow_max_smem((const void*)f, p->smem_optin) != cudaSuccess) p->fn_multi = nullptr;
@@ -314,7 +320,7 @@ static void place_multi_kernel(PinnPlan* p) {
 // Tiny batches: the (point, unit)-parallel loop kernel, for plain dense chains whose jets fit shared memory.  Left out
 // when the jet set has none (more than four directions, orders 3 / 4).
 static void place_small_kernel(PinnPlan* p) {
-    p->fn_small = nullptr; p->small_smem = 0;
+    p->fn_small = nullptr; p->small_smem = 0; p->small_budget = 0;
     const MultiKernelFn f = p->ks->small;
     if (!f) return;
     const DevPlan& h = p->h;
@@ -323,7 +329,7 @@ static void place_small_kernel(PinnPlan* p) {
     cudaFuncAttributes fs;
     if (cudaFuncGetAttributes(&fs, (const void*)f) == cudaSuccess && bytes <= p->smem_optin - (int)fs.sharedSizeBytes - 64 &&
         allow_max_smem((const void*)f, p->smem_optin) == cudaSuccess) {
-        p->fn_small = f; p->small_smem = bytes;
+        p->fn_small = f; p->small_smem = bytes; p->small_budget = p->smem_optin - (int)fs.sharedSizeBytes - 64;
     }
     (void)cudaGetLastError();
 }
@@ -788,42 +794,98 @@ extern "C" int pinn_multi_step_max_points(const PinnPlan* p) {
     return (p && p->fn_multi) ? 4096 : ((p && p->fn_small) ? 8 * pinn::small::BP : 0);
 }
 
-extern "C" int pinn_multi_step(const PinnPlan* cp, float* params, float* exp_avg, float* exp_avg_sq, const float* mask,
-                               float* step_tensors, int n_step_tensors, const float* points, const PinnColumn* cols,
-                               uint64_t seed, uint64_t* step_counter, int64_t n_points, int k_steps,
-                               float lr, float beta1, float beta2, float eps, float weight_decay, float opt_step0,
-                               float* losses_ring, int64_t ring_len, void* stream) {
+// A constraint term's plan next to the plan it trains with: the same network, parameter layout and ansatz, no
+// derivative channels, variables among the plan's.  Fills `t` (var_map: the plan's variable of every term variable).
+static int term_matches(const PinnPlan* p, const PinnPlan* q, DevTerm& t) {
+    const DevPlan& h = p->h;
+    const DevPlan& g = q->h;
+    if (g.n_layers != h.n_layers || memcmp(g.layer, h.layer, sizeof(DevLayer) * h.n_layers) != 0)
+        return fail(PINN_E_INVALID, "constraint term: its layer table differs from the plan's");
+    if (g.n_params != h.n_params || g.log_scale_off != h.log_scale_off)
+        return fail(PINN_E_INVALID, "constraint term: n_params / log_scale_off differ from the plan's");
+    if (g.nf != 0 || g.ns != 0 || spec_order(&q->spec) != 2)
+        return fail(PINN_E_INVALID, "constraint term: its plan carries derivative directions");
+    if (g.total != h.total || g.nsp != h.nsp || g.has_bc != h.has_bc || g.has_ic != h.has_ic || g.bc != h.bc ||
+        g.t0 != h.t0 || memcmp(g.lo, h.lo, sizeof(h.lo)) != 0 || memcmp(g.hi, h.hi, sizeof(h.hi)) != 0)
+        return fail(PINN_E_INVALID, "constraint term: its ansatz differs from the plan's");
+    memset(&t, 0, sizeof(t));
+    t.n_eq = g.n_eq; t.n_vars = g.n_vars;
+    for (int i = 0; i < g.n_vars; ++i) {
+        t.var_off[i] = g.var_off[i];
+        t.var_map[i] = -1;
+        for (int j = 0; j < h.n_vars; ++j) if (h.var_off[j] == g.var_off[i]) t.var_map[i] = j;
+        if (t.var_map[i] < 0) return fail(PINN_E_INVALID, "constraint term: variable %d is not one of the plan's", i);
+    }
+    for (int i = 0; i < 2 + g.n_vars; ++i) t.eq_out[i] = g.eq_out[i];     // C = 1: r, dr/du, dr/dV_i
+    memcpy(t.eq, g.eq, sizeof(t.eq));
+    return PINN_OK;
+}
+
+extern "C" int pinn_multi_step_terms(const PinnPlan* cp, float* params, float* exp_avg, float* exp_avg_sq, const float* mask,
+                                     float* step_tensors, int n_step_tensors, const float* points, const PinnColumn* cols,
+                                     uint64_t seed, uint64_t* step_counter, int64_t n_points, int k_steps,
+                                     float lr, float beta1, float beta2, float eps, float weight_decay, float opt_step0,
+                                     float* losses_ring, int64_t ring_len, float point_weight, int n_terms,
+                                     const PinnTerm* terms, void* stream) {
     PinnPlan* p = const_cast<PinnPlan*>(cp);
     if (!p || !params || !exp_avg || !exp_avg_sq || !mask || !step_counter || !losses_ring)
         return fail(PINN_E_INVALID, "null argument");
     if (!p->fn_multi && !p->fn_small) return fail(PINN_E_UNSUPPORTED, "the persistent multi-step kernels do not fit this network in shared memory");
-    if (n_points <= 0 || n_points > pinn_multi_step_max_points(p) || k_steps <= 0 || ring_len <= 0 || n_step_tensors < 0)
-        return fail(PINN_E_INVALID, "pinn_multi_step: n_points %lld (1..%d), k_steps %d", (long long)n_points, pinn_multi_step_max_points(p), k_steps);
+    if (n_terms < 0 || n_terms > PINN_MAX_TERMS || (n_terms > 0 && !terms))
+        return fail(PINN_E_INVALID, "pinn_multi_step_terms: %d terms (0..%d)", n_terms, PINN_MAX_TERMS);
+    if (!(point_weight >= 0.0f) || point_weight > 3.0e38f) return fail(PINN_E_INVALID, "point_weight must be finite and >= 0");
+    MultiArgs a;
+    memset(&a.terms, 0, sizeof(a.terms));
+    a.terms.n_terms = n_terms;
+    int rows = p->h.rows_total, n_slots = p->h.n_slots;             // scratch rows: the most any program needs
+    for (int t = 0; t < n_terms; ++t) {
+        const PinnTerm& T = terms[t];
+        if (!T.plan || !T.points || T.n_points < 1 || a.terms.n_points + T.n_points > PINN_MAX_TERM_POINTS)
+            return fail(PINN_E_INVALID, "constraint term %d: null plan / points, or more than %d points in all", t, PINN_MAX_TERM_POINTS);
+        if (!(T.point_weight >= 0.0f) || T.point_weight > 3.0e38f) return fail(PINN_E_INVALID, "constraint term %d: point_weight", t);
+        DevTerm& d = a.terms.t[t];
+        const int rc = term_matches(p, T.plan, d);
+        if (rc) return rc;
+        d.weight = T.point_weight;
+        a.terms.first[t] = a.terms.n_points;
+        for (int i = 0; i < T.n_points; ++i)
+            for (int k = 0; k < p->h.total; ++k) a.terms.x[a.terms.n_points + i][k] = T.points[(size_t)i * p->h.total + k];
+        a.terms.n_points += T.n_points;
+        if (T.plan->h.n_slots > n_slots) n_slots = T.plan->h.n_slots;
+        if (p->h.row_scr + T.plan->h.n_slots > rows) rows = p->h.row_scr + T.plan->h.n_slots;
+    }
+    a.terms.first[n_terms] = a.terms.n_points;
+    const long long n_cols = n_points + a.terms.n_points;
+    if (n_points <= 0 || n_cols > pinn_multi_step_max_points(p) || k_steps <= 0 || ring_len <= 0 || n_step_tensors < 0)
+        return fail(PINN_E_INVALID, "pinn_multi_step: n_points %lld + %d constraint points (1..%d), k_steps %d", (long long)n_points,
+                    a.terms.n_points, pinn_multi_step_max_points(p), k_steps);
     if (!aligned16(params)) return fail(PINN_E_ALIGN, "params must be 16-byte aligned");
     DevPlan plan = p->h;
+    plan.n_slots = n_slots;                                         // the small kernel's scratch rows
     if (!points) { int rc = resolve_cols(p, cols, plan.cols); if (rc) return rc; }
-    MultiArgs a;
     a.params = params; a.exp_avg = exp_avg; a.exp_avg_sq = exp_avg_sq; a.mask = mask;
     a.step_tensors = step_tensors; a.n_step_tensors = n_step_tensors; a.points = points; a.seed = seed;
     a.step_counter = reinterpret_cast<unsigned long long*>(step_counter);
-    a.n_points = n_points; a.inv_n = 1.0f / (float)n_points; a.k_steps = k_steps;
+    a.n_points = n_points; a.inv_n = point_weight; a.k_steps = k_steps;
     a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = weight_decay; a.opt_step0 = opt_step0;
     a.losses_ring = losses_ring; a.ring_len = ring_len;
-    a.rows_total = p->h.rows_total;
+    a.rows_total = rows;
     // batches of at most 128 points: the (point, unit)-parallel kernel (PINN_MULTI_KERNEL=tile forces the other one)
     const char* mk = getenv("PINN_MULTI_KERNEL");
-    const bool small_ok = p->fn_small && n_points <= 8 * pinn::small::BP && (n_points <= 256 || !p->fn_multi) &&
+    const bool small_ok = p->fn_small && n_cols <= 8 * pinn::small::BP && (n_cols <= 256 || !p->fn_multi) &&
                           !(mk && !strcmp(mk, "tile") && p->fn_multi);
     if (small_ok) {
-        // a cluster of up to 8 CTAs (8 SMs) shares the batch, ~16 points per CTA at least; PINN_SMALL_CLUSTER overrides
-        int nc = (int)((n_points + 15) / 16);
+        const int smem = n_slots == p->h.n_slots ? p->small_smem : small::make_layout(plan).total * 4;
+        if (smem > p->small_budget) return fail(PINN_E_UNSUPPORTED, "the constraint programs' scratch slots do not fit shared memory");
+        // a cluster of up to 8 CTAs (8 SMs) shares the columns, ~16 per CTA at least; PINN_SMALL_CLUSTER overrides
+        int nc = (int)((n_cols + 15) / 16);
         if (nc > 8) nc = 8;
         { const char* e = getenv("PINN_SMALL_CLUSTER"); if (e && atoi(e) >= 1 && atoi(e) <= 8) nc = atoi(e); }
-        while ((n_points + nc - 1) / nc > pinn::small::BP) ++nc;
+        while ((n_cols + nc - 1) / nc > pinn::small::BP) ++nc;
         if (nc == 3) nc = 4; else if (nc > 4 && nc < 8) nc = 8;         // cluster sizes 1, 2, 4, 8
         cudaLaunchConfig_t cfg;
         memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = dim3(nc); cfg.blockDim = dim3(pinn::small::NT); cfg.dynamicSmemBytes = p->small_smem;
+        cfg.gridDim = dim3(nc); cfg.blockDim = dim3(pinn::small::NT); cfg.dynamicSmemBytes = smem;
         cfg.stream = (cudaStream_t)stream;
         cudaLaunchAttribute attr[1];
         attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -831,10 +893,22 @@ extern "C" int pinn_multi_step(const PinnPlan* cp, float* params, float* exp_avg
         cfg.attrs = attr; cfg.numAttrs = 1;
         CUDA_TRY(cudaLaunchKernelEx(&cfg, p->fn_small, plan, a));
     } else {
-        p->fn_multi<<<1, p->multi_threads, p->multi_smem, (cudaStream_t)stream>>>(plan, a);
+        const int smem = rows == p->h.rows_total ? p->multi_smem : multi_smem_bytes(p->h, p->multi_threads / 32, rows);
+        if (smem > p->multi_budget) return fail(PINN_E_UNSUPPORTED, "the constraint programs' scratch slots do not fit shared memory");
+        p->fn_multi<<<1, p->multi_threads, smem, (cudaStream_t)stream>>>(plan, a);
     }
     CUDA_TRY(cudaGetLastError());
     return PINN_OK;
+}
+
+extern "C" int pinn_multi_step(const PinnPlan* p, float* params, float* exp_avg, float* exp_avg_sq, const float* mask,
+                               float* step_tensors, int n_step_tensors, const float* points, const PinnColumn* cols,
+                               uint64_t seed, uint64_t* step_counter, int64_t n_points, int k_steps,
+                               float lr, float beta1, float beta2, float eps, float weight_decay, float opt_step0,
+                               float* losses_ring, int64_t ring_len, void* stream) {
+    return pinn_multi_step_terms(p, params, exp_avg, exp_avg_sq, mask, step_tensors, n_step_tensors, points, cols, seed,
+                                 step_counter, n_points, k_steps, lr, beta1, beta2, eps, weight_decay, opt_step0,
+                                 losses_ring, ring_len, n_points > 0 ? 1.0f / (float)n_points : 0.0f, 0, nullptr, stream);
 }
 
 extern "C" int pinn_forward(const PinnPlan* p, const float* params, const float* points, int64_t n_points,

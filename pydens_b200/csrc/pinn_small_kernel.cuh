@@ -18,6 +18,10 @@
 //
 // Covered: batches of at most 128 points per CTA (1024 per launch), dense chains without residual wiring whose state
 // fits shared memory (everything the README / tutorial problems need).  Selected by pinn_multi_step for such batches.
+//
+// Constraint terms (pinn_multi_step_terms, a.terms): their fixed points are columns n_points .. n_points + a.terms.n_points - 1
+// behind the batch, split over the CTAs with it.  Such a column runs the same forward jets; in the residual phase it
+// evaluates its term's program on the value channel, with the term's weight and zero seeds on the derivative channels.
 #pragma once
 
 #include <cooperative_groups.h>
@@ -59,7 +63,7 @@ __host__ __device__ inline Layout make_layout(const DevPlan& P) {
 }
 
 template <int NF, int NS>
-__global__ void __launch_bounds__(NT, 1) small_step_kernel(const __grid_constant__ DevPlan P, const MultiArgs a) {
+__global__ void __launch_bounds__(NT, 1) small_step_kernel(const __grid_constant__ DevPlan P, const __grid_constant__ MultiArgs a) {
     constexpr int C = 1 + NF + NS;
     extern __shared__ __align__(16) float smem[];
     const int tid = threadIdx.x, lane = tid & 31;
@@ -74,10 +78,11 @@ __global__ void __launch_bounds__(NT, 1) small_step_kernel(const __grid_constant
     float* gsum = smem + Y.gsum;
     const int Ln = P.n_layers;
     const int n_out_floats = P.n_params + 4;
-    // this CTA's slice of the batch
+    // this CTA's slice of the columns: the batch, then the constraint terms' points
     cg::cluster_group cluster = cg::this_cluster();
     const int crank = (int)cluster.block_rank(), csize = (int)cluster.num_blocks();
-    const int q_pts = (int)a.n_points / csize, r_pts = (int)a.n_points % csize;
+    const int n_cols = (int)a.n_points + a.terms.n_points;
+    const int q_pts = n_cols / csize, r_pts = n_cols % csize;
     const int B = q_pts + (crank < r_pts ? 1 : 0);                       // points of this CTA (may be 0)
     const int base = crank * q_pts + (crank < r_pts ? crank : r_pts);    // index of its first point in the batch
     const int Bp = (B + 3) & ~3;
@@ -94,7 +99,9 @@ __global__ void __launch_bounds__(NT, 1) small_step_kernel(const __grid_constant
         // ---- the batch: coordinates of point p in X[k][p]; padded points replay the last one (their adjoint seed is 0)
         if (tid < BP && B > 0) {
             const int p = tid, pe = base + (p < B ? p : B - 1);
-            if (a.points) {
+            if (pe >= a.n_points) {                                      // a constraint point: fixed, no sampler draw
+                for (int k = 0; k < P.total; ++k) X[k * SR + p] = a.terms.x[pe - a.n_points][k];
+            } else if (a.points) {
                 const float* src = a.points + ((size_t)s * a.n_points + (size_t)pe) * P.total;
                 for (int k = 0; k < P.total; ++k) X[k * SR + p] = __ldg(src + k);
             } else {
@@ -171,6 +178,8 @@ __global__ void __launch_bounds__(NT, 1) small_step_kernel(const __grid_constant
         if (tid < Bp) {
             const int p = tid;
             const bool valid = p < B;
+            const int q = base + (valid ? p : B - 1);            // its column (a padded one replays the last)
+            const DevTerm* term = q >= a.n_points ? &a.terms.t[term_of(a.terms, q - (int)a.n_points)] : nullptr;
             float* nrow = smem + Y.lev[Ln] + p;                  // level Ln: one unit, C channels
             float N[C];
 #pragma unroll
@@ -188,26 +197,42 @@ __global__ void __launch_bounds__(NT, 1) small_step_kernel(const __grid_constant
             AnsatzState<NF, NS> as;
             float u[C];
             ansatz_forward<NF, NS, true>(P, coords, SR, flat[P.log_scale_off], N, icj, as, u);
-#pragma unroll
-            for (int c = 0; c < C; ++c) sc[(size_t)c * SR] = u[c];
-            eval_prog(P.eq, P.n_eq, sc, SR, coords, flat, P.var_off);
-            const float r = sc[(size_t)P.eq_out[0] * SR];
-            const float rb = valid ? 2.0f * r * a.inv_n : 0.0f;
-            red[0 * SR + p] = valid ? r * a.inv_n * r : 0.0f;
             float ub[C];
+            if (term) {
+                float icv[PINN_MAX_VARS];
+                term_ic_partials<NF, NS>(P, sc, SR, icv);
+                sc[0] = u[0];
+                eval_prog(term->eq, term->n_eq, sc, SR, coords, flat, term->var_off);
+                const float r = sc[(size_t)term->eq_out[0] * SR];
+                const float rb = valid ? 2.0f * r * term->weight : 0.0f;
+                red[0 * SR + p] = valid ? r * term->weight * r : 0.0f;
+                PointPartials<NF, NS> part;
 #pragma unroll
-            for (int c = 0; c < C; ++c) ub[c] = rb * sc[(size_t)P.eq_out[1 + c] * SR];
+                for (int i = 0; i < PINN_MAX_VARS; ++i) part.vbar[i] = 0.0f;
+                term_seeds<NF, NS>(P, *term, sc, SR, rb, icv, ub, part);
 #pragma unroll
-            for (int i = 0; i < PINN_MAX_VARS; ++i) {
-                float v = 0.0f;
-                if (i < P.n_vars) {
-                    v = rb * sc[(size_t)P.eq_out[1 + C + i] * SR];
-                    if (P.ic_has_vars) {
+                for (int i = 0; i < PINN_MAX_VARS; ++i) red[(2 + i) * SR + p] = part.vbar[i];
+            } else {
 #pragma unroll
-                        for (int c = 0; c < C; ++c) v = fmaf(ub[c], sc[(size_t)P.ic_out[C * (1 + i) + c] * SR], v);
+                for (int c = 0; c < C; ++c) sc[(size_t)c * SR] = u[c];
+                eval_prog(P.eq, P.n_eq, sc, SR, coords, flat, P.var_off);
+                const float r = sc[(size_t)P.eq_out[0] * SR];
+                const float rb = valid ? 2.0f * r * a.inv_n : 0.0f;
+                red[0 * SR + p] = valid ? r * a.inv_n * r : 0.0f;
+#pragma unroll
+                for (int c = 0; c < C; ++c) ub[c] = rb * sc[(size_t)P.eq_out[1 + c] * SR];
+#pragma unroll
+                for (int i = 0; i < PINN_MAX_VARS; ++i) {
+                    float v = 0.0f;
+                    if (i < P.n_vars) {
+                        v = rb * sc[(size_t)P.eq_out[1 + C + i] * SR];
+                        if (P.ic_has_vars) {
+#pragma unroll
+                            for (int c = 0; c < C; ++c) v = fmaf(ub[c], sc[(size_t)P.ic_out[C * (1 + i) + c] * SR], v);
+                        }
                     }
+                    red[(2 + i) * SR + p] = v;
                 }
-                red[(2 + i) * SR + p] = v;
             }
             float Nb[C];
             red[1 * SR + p] = ansatz_adjoint<NF, NS>(P, as, ub, Nb);

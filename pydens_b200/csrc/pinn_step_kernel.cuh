@@ -539,8 +539,10 @@ __global__ void __launch_bounds__(MAXT, 1) coupled_step_kernel(const __grid_cons
 // whole optimizer steps per launch.  Parameters, Adam moments and the gradient live in shared memory
 // between the steps; every step is  sample / read points -> forward jets -> residual -> reverse ->
 // CTA-wide fixed-order reduction -> Adam (torch.optim.Adam semantics, fused/capturable form) -> re-layout
-// of the weights, with no launch and no trip to global memory in between.  Opt-in:
-// Solver.fit(..., steps_per_launch=k).
+// of the weights, with no launch and no trip to global memory in between.  Solver.fit takes it by itself for tiny
+// batches, or with steps_per_launch=k.  Constraint terms (pinn_multi_step_terms) travel by value in MultiArgs::terms:
+// their points are one more tile, walked after the batch tiles, whose lanes run the terms' residual programs.
+// MultiArgs is a __grid_constant__ parameter of both persistent kernels, so that a term is read in place, by address.
 // ---------------------------------------------------------------------------------------------------
 struct MultiArgs {
     float* params;                 // [n_params] in/out
@@ -553,17 +555,20 @@ struct MultiArgs {
     uint64_t seed;
     unsigned long long* step_counter;   // device step number (Philox counter word, ring index); += k_steps
     long long n_points;
-    float inv_n;
+    float inv_n;                   // the point weight of the batch: 1 / n_points, or 1 for reduction='sum'
     int k_steps;
     float lr, beta1, beta2, eps, weight_decay;
     float opt_step0;               // optimizer steps taken before this launch
     float* losses_ring;
     long long ring_len;
     int rows_total;
+    DevTerms terms;                // constraint terms (terms.n_terms = 0: none)
 };
+// kernel parameters are limited to 32764 bytes (CUDA 12.1+ on Hopper); 16 bytes for the alignment of the second one
+static_assert(sizeof(DevPlan) + sizeof(MultiArgs) + 16 <= 32764, "DevPlan + MultiArgs exceed the kernel-parameter limit");
 
 template <int NF, int NS, int MAXT, int JF>
-__global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_constant__ DevPlan P, const MultiArgs a) {
+__global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_constant__ DevPlan P, const __grid_constant__ MultiArgs a) {
     extern __shared__ __align__(16) float smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
     const int n_out_floats = P.n_params + 4;
@@ -597,21 +602,32 @@ __global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_consta
         part.loss = 0.0f; part.sbar = 0.0f;
 #pragma unroll
         for (int i = 0; i < PINN_MAX_VARS; ++i) part.vbar[i] = 0.0f;
-        for (long long tile = warp; tile < n_tiles; tile += nwarps) {
-            const long long pl = tile * 32 + lane;
-            const bool valid = pl < a.n_points;
-            const long long pe = valid ? pl : a.n_points - 1;
-            if (a.points) {
-                const float* src = a.points + ((size_t)s * a.n_points + (size_t)pe) * P.total;
-                for (int k = 0; k < P.total; ++k) st[k * RS] = __ldg(src + k);
+        // the batch tiles, then one tile of the constraint terms' points (at most 32); its masked lanes replay its last point
+        const long long n_walk = n_tiles + (a.terms.n_points > 0 ? 1 : 0);
+        for (long long tile = warp; tile < n_walk; tile += nwarps) {
+            const DevTerm* term = nullptr;
+            bool valid;
+            if (tile < n_tiles) {
+                const long long pl = tile * 32 + lane;
+                valid = pl < a.n_points;
+                const long long pe = valid ? pl : a.n_points - 1;
+                if (a.points) {
+                    const float* src = a.points + ((size_t)s * a.n_points + (size_t)pe) * P.total;
+                    for (int k = 0; k < P.total; ++k) st[k * RS] = __ldg(src + k);
+                } else {
+                    const uint64_t gidx = (uint64_t)pe;
+                    Philox4 b0 = philox_block(gidx, step, a.seed, 0u);
+                    Philox4 b1 = b0;
+                    if (P.total > 4) b1 = philox_block(gidx, step, a.seed, 1u);
+                    for (int k = 0; k < P.total; ++k) st[k * RS] = sample_column(P.cols[k], k, gidx, step, a.seed, b0, b1);
+                }
             } else {
-                const uint64_t gidx = (uint64_t)pe;
-                Philox4 b0 = philox_block(gidx, step, a.seed, 0u);
-                Philox4 b1 = b0;
-                if (P.total > 4) b1 = philox_block(gidx, step, a.seed, 1u);
-                for (int k = 0; k < P.total; ++k) st[k * RS] = sample_column(P.cols[k], k, gidx, step, a.seed, b0, b1);
+                valid = lane < a.terms.n_points;
+                const int q = valid ? lane : a.terms.n_points - 1;
+                for (int k = 0; k < P.total; ++k) st[k * RS] = a.terms.x[q][k];
+                term = &a.terms.t[term_of(a.terms, q)];
             }
-            point_step<NF, NS, JF, true>(P, sw, flat, st, RS, valid, a.inv_n, sink, part);
+            point_step<NF, NS, JF, true, false, true>(P, sw, flat, st, RS, valid, a.inv_n, sink, part, term);
         }
         {
             float v = warp_sum(part.loss);

@@ -233,7 +233,7 @@ class FusedEngine:
                     ws = torch.zeros(self.lib.pinn_workspace_bytes(plan, 1), dtype=torch.uint8, device=self.device)
                     entry = dict(plan=plan, spec=spec, points=pts.to(self.device).contiguous(), n=int(pts.shape[0]),
                                  out=torch.zeros(self.n_params + 4, dtype=torch.float32, device=self.device),
-                                 workspace=ws)
+                                 workspace=ws, host_points=pts.detach().cpu().contiguous())
                 elif rc != _native.E_UNSUPPORTED:
                     _native.check(rc)
             self._constraint_plans[num] = entry
@@ -405,10 +405,35 @@ class FusedEngine:
         self._adam_bound_to, self._adam_bound_sig = opt, sig
         return mask
 
-    def _fit_persistent(self, niters, batch_size, sampler, opt, k):
-        """ `niters` optimizer steps, `k` per launch of the persistent multi-step kernel (pinn_multi_step):
-        the reference loop model_torch.py:426-464 with optimizer.step() inside the kernel. """
+    def _persistent_terms(self, loss_terms, batch_size):
+        """ The constraint terms of a fit as terms of the persistent kernels (pinn_multi_step_terms): a list of
+        constraint plans, or None when the fit has no equation term, or a constraint that does not lower to a fused
+        plan, or more terms / constraint points than the kernels take. """
+        if 'equation' not in loss_terms:
+            return None
+        entries = [self._constraint_plan(n) for n in self.solver._constraint_numbers(loss_terms)]
+        if any(e is None for e in entries) or len(entries) > _native.MAX_TERMS:
+            return None
+        if sum(e['n'] for e in entries) > _native.MAX_TERM_POINTS:
+            return None
+        if batch_size + sum(e['n'] for e in entries) > self.lib.pinn_multi_step_max_points(self.plan):
+            return None
+        return entries
+
+    def _fit_persistent(self, niters, batch_size, sampler, opt, k, terms=()):
+        """ `niters` optimizer steps, `k` per launch of the persistent multi-step kernel (pinn_multi_step_terms):
+        the reference loop model_torch.py:426-464 with optimizer.step() inside the kernel, constraint terms included.
+        Returns False, having taken no step, when the kernels cannot hold the constraint programs' scratch slots. """
         solver = self.solver
+        # point weights: the mean of model_torch.py:448 over the batch and over every constraint's own points, or 1
+        total_sum = self._sum_reduction()
+        term_arr = (_native.PinnTerm * max(1, len(terms)))()
+        for i, e in enumerate(terms):
+            term_arr[i].plan = e['plan'].value
+            term_arr[i].n_points = e['n']
+            term_arr[i].point_weight = 1.0 if total_sum else 1.0 / e['n']
+            term_arr[i].points = e['host_points'].data_ptr()
+        point_weight = 1.0 if total_sum else 1.0 / batch_size
         total = solver.model.total
         g = opt.param_groups[0]
         mask = self._bind_adam_state(opt)
@@ -445,19 +470,24 @@ class FusedEngine:
                     b = host_sampler.sample(batch_size)
                     host[j].copy_(b if isinstance(b, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(b, dtype=np.float32)))
                 pts = host.to(self.device, non_blocking=True)
-            _native.check(self.lib.pinn_multi_step(
+            rc = self.lib.pinn_multi_step_terms(
                 self.plan, C.c_void_p(self.flat.data_ptr()), C.c_void_p(m.data_ptr()), C.c_void_p(v.data_ptr()),
                 C.c_void_p(mask.data_ptr()), C.c_void_p(steps.data_ptr()), C.c_int(steps.numel()),
                 C.c_void_p(pts.data_ptr()) if pts is not None else None, cols, C.c_uint64(self.seed),
                 C.c_void_p(self.step_counter.data_ptr()), C.c_int64(batch_size), C.c_int(kk),
                 C.c_float(lr), C.c_float(b1), C.c_float(b2), C.c_float(g['eps']), C.c_float(g['weight_decay']),
-                C.c_float(opt_step0 + done), C.c_void_p(ring.data_ptr()), C.c_int64(ring_len), self._stream()))
+                C.c_float(opt_step0 + done), C.c_void_p(ring.data_ptr()), C.c_int64(ring_len),
+                C.c_float(point_weight), C.c_int(len(terms)), term_arr, self._stream())
+            if rc == _native.E_UNSUPPORTED and done == 0 and terms:
+                return False
+            _native.check(rc)
             done += kk
         self.steps_done = start + niters
         torch.cuda.synchronize(self.device)
         idx = (start + np.arange(drained, niters)) % ring_len
         vals[drained:niters] = ring.cpu().numpy()[idx]
         solver.losses.extend(np.array(x, dtype=np.float32) for x in vals)
+        return True
 
     def fit(self, niters, batch_size, sampler, loss_terms, optimizer, criterion, lr, **kwargs):
         solver = self.solver
@@ -473,22 +503,28 @@ class FusedEngine:
             steps_per_launch = _AUTO_PERSISTENT_STEPS
         if steps_per_launch > 0 and niters > 0:
             g = opt.param_groups[0] if opt.param_groups else {}
-            ok = (type(opt) is torch.optim.Adam and len(opt.param_groups) == 1 and not g.get('amsgrad') and not g.get('maximize')
-                  and not torch.is_tensor(g.get('lr')) and not self._sum_reduction()
-                  and _dist() is None and not solver._constraint_numbers(loss_terms)
-                  and 0 < batch_size <= self.lib.pinn_multi_step_max_points(self.plan))
+            terms = None
+            if (type(opt) is torch.optim.Adam and len(opt.param_groups) == 1 and not g.get('amsgrad') and not g.get('maximize')
+                    and not torch.is_tensor(g.get('lr')) and _dist() is None and batch_size > 0):
+                terms = self._persistent_terms(loss_terms, batch_size)
+            ok = terms is not None
             if not ok and not requested:
                 steps_per_launch = 0
             elif ok:
                 if solver.optimizer is not self._opt_obj:
                     self._drop_graphs()
                     self._opt_obj, self._opt_key = solver.optimizer, None
-                return self._fit_persistent(niters, batch_size, sampler, opt, steps_per_launch)
+                if self._fit_persistent(niters, batch_size, sampler, opt, steps_per_launch, terms):
+                    return
+                if not requested:
+                    steps_per_launch = 0
         if steps_per_launch > 0 and niters > 0:
             import warnings
-            warnings.warn('pydens_b200: steps_per_launch ignored (needs Adam, one device, no constraints, a batch of at '
-                          'most %d points and a network that fits the persistent kernel)'
-                          % self.lib.pinn_multi_step_max_points(self.plan), stacklevel=3)
+            warnings.warn('pydens_b200: steps_per_launch ignored (needs Adam, one device, the equation term, constraints '
+                          'that run fused (at most %d, with %d points in all), batch + constraint points of at most %d '
+                          'and a network that fits the persistent kernel)'
+                          % (_native.MAX_TERMS, _native.MAX_TERM_POINTS, self.lib.pinn_multi_step_max_points(self.plan)),
+                          stacklevel=3)
         if solver.optimizer is not self._opt_obj:          # optimizer=None with an optimizer built elsewhere
             self._drop_graphs()
             self._opt_obj, self._opt_key = solver.optimizer, None

@@ -304,7 +304,8 @@ class Solver:
                     steps_per_launch=k  (fused path, small batches): k whole optimizer steps — Adam included — per
                     launch of a persistent kernel.  Batches of at most 1024 points (the launch-bound regime of the
                     README example, batch_size=100, niters=1500) take this path by themselves, 50 steps per launch,
-                    whenever the optimizer is plain Adam, there is one device and no constraint term
+                    whenever the optimizer is plain Adam, there is one device, the equation is a loss term and every
+                    constraint term runs fused (at most 4 of them, 32 constraint points in all)
                     (PYDENS_B200_AUTO_PERSISTENT=0 keeps one launch per step).
         """
         loss_terms = loss_terms if isinstance(loss_terms, (tuple, list)) else (loss_terms,)
