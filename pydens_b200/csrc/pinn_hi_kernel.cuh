@@ -18,8 +18,6 @@ __global__ void __launch_bounds__(256, 1) hi_step_kernel(const __grid_constant__
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
     const int n_out_floats = P.n_params + 4;
     const SmemLayout SL = smem_layout(P.weights_floats, n_out_floats, a.wacc ? 0 : nwarps, P.n_params);
-    pdl_wait();
-    pdl_launch_dependents();
     stage_weights(smem, SL, P, a.params);
     const float* sw = smem + SL.weights_f;
     float* wacc_all = warp_accumulators(a, smem, SL, n_out_floats, nwarps);

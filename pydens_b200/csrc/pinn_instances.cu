@@ -52,20 +52,18 @@ void enter() {
     k.step[1][1] = hi::hi_step_kernel<NF, J>;
     k.maxt = 256;
 #elif PINN_UNIT == PINN_WIDE
-    KernelSet& k = kernel_slot(NF, J, 2);
-    k.wide[0] = wide::wide_step_kernel<NF, J, 512>;
-    k.wide[1] = wide::wide_step_kernel<NF, J, 256>;
+    kernel_slot(NF, J, 2).wide = wide::wide_step_kernel<NF, J>;
 #elif PINN_UNIT == PINN_WIDE128
     kernel_slot(NF, J, 2).wide128 = wide::wide128_step_kernel<NF, J>;
 #elif PINN_UNIT == PINN_SMALL
     kernel_slot(NF, J, 2).small = small::small_step_kernel<NF, J>;
 #elif PINN_UNIT == PINN_COUPLED
     using Cfg = VariantCfg<NF, J>;
-    CoupledSet& k = coupled_slot(NF, J);
-    k.step[0] = coupled_step_kernel<NF, J, false, Cfg::MAXT>;
-    k.step[1] = coupled_step_kernel<NF, J, true, Cfg::MAXT>;
+    KernelSet& k = kernel_slot(NF, J, 2);
+    k.coupled[0] = coupled_step_kernel<NF, J, false, Cfg::MAXT>;
+    k.coupled[1] = coupled_step_kernel<NF, J, true, Cfg::MAXT>;
 #elif PINN_UNIT == PINN_WIDE128_COUPLED
-    coupled_slot(NF, J).wide128 = wide::wide128_coupled_step_kernel<NF, J>;
+    kernel_slot(NF, J, 2).coupled_wide128 = wide::wide128_coupled_step_kernel<NF, J>;
 #else
 #error "PINN_UNIT names no kernel family"
 #endif

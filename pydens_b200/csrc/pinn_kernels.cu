@@ -40,17 +40,6 @@ const KernelSet* kernels(int nf, int ns, int order) {
     return k.step[1][1] ? &k : nullptr;
 }
 
-CoupledSet& coupled_slot(int nf, int ns) {
-    static CoupledSet table[5][5];                                     // [nf][ns]
-    return table[nf][ns];
-}
-
-const CoupledSet* coupled_kernels(int nf, int ns) {
-    if (nf < 0 || nf > 4 || ns < 0 || ns > nf) return nullptr;
-    const CoupledSet& k = coupled_slot(nf, ns);
-    return k.step[1] ? &k : nullptr;
-}
-
 // ---------------------------------------------------------------------------------------------------
 // Forward-only kernel (predict): u for explicit points; MULTI: the k components of every point, u_out [n_points, k].
 // ---------------------------------------------------------------------------------------------------
@@ -95,11 +84,11 @@ __global__ void __launch_bounds__(256, 1) coupled_forward_kernel(const __grid_co
 
 // The forward-only form of the 128-wide tile kernel (declared in pinn_wide_kernel.cuh).
 __global__ void __launch_bounds__(512, 1) wide::wide128_forward_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
-    wide::wide_step<0, 0, 512, 128, true>(P, a);
+    wide::wide_step<0, 0, 128, true>(P, a);
 }
 // ... and of its coupled form: u_out [n, k]
 __global__ void __launch_bounds__(512, 1) wide::wide128_coupled_forward_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
-    wide::wide_step<0, 0, 512, 128, true, true>(P, a);
+    wide::wide_step<0, 0, 128, true, true>(P, a);
 }
 
 // Points the in-kernel sampler produces (for tests / replay).
@@ -343,8 +332,7 @@ static int place_wide_kernel(PinnPlan* p, int order, int thread_rc) {
     const char* fk = getenv("PINN_FORCE_KERNEL");
     const bool eligible = order < 3 && wide_eligible(p->h, &mw);
     // networks of 2..4 outputs: the coupled form of the 128-wide class only
-    const CoupledSet* cs = p->coupled ? coupled_kernels(p->h.nf, p->h.ns) : nullptr;
-    const StepKernelFn f128 = p->coupled ? (cs ? cs->wide128 : nullptr) : p->ks->wide128;
+    const StepKernelFn f128 = p->coupled ? p->ks->coupled_wide128 : p->ks->wide128;
     const bool eligible64 = eligible && !p->coupled;
     const bool eligible128 = eligible && mw > 64 && f128;
     // the tile kernel wins from 64-wide layers with many jet channels on (H100 80GB HBM3 at 700 W, cfg5: 21.1 ms
@@ -363,9 +351,7 @@ static int place_wide_kernel(PinnPlan* p, int order, int thread_rc) {
         if (!eligible128) return fail(PINN_E_UNSUPPORTED, "PINN_FORCE_KERNEL=wide128: this network is outside what the 128-wide tile kernel covers");
         want = true; kw = 128;
     }
-    int wide_threads = 512;                     // four threads per point; PINN_WIDE_THREADS=256: two (experiments, 64-wide class)
-    { const char* wt = getenv("PINN_WIDE_THREADS"); if (wt && atoi(wt) == 256 && kw == 64) wide_threads = 256; }
-    const StepKernelFn f = kw == 128 ? f128 : p->ks->wide[wide_threads == 256 ? 1 : 0];
+    const StepKernelFn f = kw == 128 ? f128 : p->ks->wide;
     if (!want || !f || (thread_rc != PINN_OK && kw != 128)) return thread_rc;
     const int smem = kw == 128 ? (p->coupled ? wide::Tile<128, true>::SMEM_BYTES : wide::Tile<128>::SMEM_BYTES)
                                : wide::Tile<64>::SMEM_BYTES;
@@ -375,7 +361,7 @@ static int place_wide_kernel(PinnPlan* p, int order, int thread_rc) {
     e = cudaFuncGetAttributes(&fa, (const void*)f);
     if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncGetAttributes(wide): %s", cudaGetErrorString(e));
     p->fn_wide = f;
-    p->wide = true; p->wide_kw = kw; p->gmem = true; p->threads = wide_threads; p->wacc_gmem = false;
+    p->wide = true; p->wide_kw = kw; p->gmem = true; p->threads = wide::NT; p->wacc_gmem = false;
     p->smem_bytes = smem; p->regs = fa.numRegs;
     if (thread_rc != PINN_OK) {                 // the forward kernel does not hold this network either
         const void* ff = p->coupled ? (const void*)wide::wide128_coupled_forward_kernel : (const void*)wide::wide128_forward_kernel;
@@ -410,10 +396,9 @@ extern "C" int pinn_plan_create(const PinnSpec* s, int device, PinnPlan** out) {
     // networks of 2..4 outputs: their own step kernels (build_dev_plan has refused what those do not cover)
     p->coupled = p->h.layer[p->h.n_layers - 1].n_out > 1;
     if (p->coupled) {
-        const CoupledSet* cs = coupled_kernels(p->h.nf, p->h.ns);
-        if (!cs) return fail(PINN_E_UNSUPPORTED, "no kernel for a network of several outputs with nf=%d ns=%d", p->h.nf, p->h.ns);
-        p->fn_smem = cs->step[0];
-        p->fn_gmem = cs->step[1];
+        if (!p->ks->coupled[1]) return fail(PINN_E_UNSUPPORTED, "no kernel for a network of several outputs with nf=%d ns=%d", p->h.nf, p->h.ns);
+        p->fn_smem = p->ks->coupled[0];
+        p->fn_gmem = p->ks->coupled[1];
     }
     p->spec = *s;
     p->device = device;
@@ -679,21 +664,10 @@ extern "C" int pinn_pipe_sync(PinnPipe* q) {
     return PINN_OK;
 }
 
-// PINN_PDL=1 launches the step kernels with programmatic stream serialization (the kernel itself waits for its
-// predecessor, griddepcontrol.wait, before it reads anything the predecessor wrote).  Graph-replayed steps (what
-// `fit` runs) have no launch gap for it to hide, so it stays opt-in.
 static int launch_step(StepKernelFn fn, int grid, int threads, int smem_bytes, cudaStream_t st, const DevPlan& plan,
                        const StepArgs& a) {
-    static int pdl = -1;
-    if (pdl < 0) { const char* e = getenv("PINN_PDL"); pdl = (e && !strcmp(e, "1")) ? 1 : 0; }
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = (size_t)smem_bytes; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-    CUDA_TRY(cudaLaunchKernelEx(&cfg, fn, plan, a));
+    fn<<<grid, threads, smem_bytes, st>>>(plan, a);
+    CUDA_TRY(cudaGetLastError());
     return PINN_OK;
 }
 

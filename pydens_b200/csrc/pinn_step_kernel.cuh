@@ -201,13 +201,6 @@ __device__ __forceinline__ float fold_column(const float* __restrict__ src, int 
     return (s0 + s1) + (s2 + s3);
 }
 
-// Programmatic dependent launch: consecutive steps are launched with programmatic stream serialization, so the CTAs of
-// step s+1 are placed on the SMs as the CTAs of step s drain (fold, all-reduce and Adam run in ONE last CTA) instead
-// of after the whole grid has retired.  pdl_wait() blocks until the previous grid has completed and its writes
-// (parameters, step counter, ticket words) are visible; without the launch attribute both are no-ops.
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
 // optimizer.step() (reference model_torch.py:461) inside the step kernel: torch.optim.Adam's update, element by element,
 // applied by the thread that has just produced the reduced gradient element.
 struct AdamHyper { float step_size, bc2_sqrt; };
@@ -441,8 +434,6 @@ __device__ __forceinline__ void step_body(const DevPlan& P, const StepArgs& a) {
     const int n_out_floats = P.n_params + 4;
     const SmemLayout SL = smem_layout(P.weights_floats, n_out_floats, a.wacc ? 0 : nwarps,
                                       GMEM ? P.n_params : max(P.n_params, a.rows_total * RS * nwarps));
-    pdl_wait();                                    // the previous step (its parameter update) is complete and visible
-    pdl_launch_dependents();                       // the next step's CTAs may take the SMs as ours leave them
     stage_weights(smem, SL, P, a.params);
     const float* sw = smem + SL.weights_f;
     float* wacc_all = warp_accumulators(a, smem, SL, n_out_floats, nwarps);
@@ -698,20 +689,13 @@ struct KernelSet {
                                              // hi_step_kernel), which serves plain plans too.
     MultiKernelFn multi;                     // persistent multi-step kernel (general form, smem-resident)
     MultiKernelFn small;                     // tiny-batch cluster kernel (pinn_small_kernel.cuh)
-    StepKernelFn wide[2];                    // tensor-core tile kernel (pinn_wide_kernel.cuh), [0]: 512, [1]: 256 threads
+    StepKernelFn wide;                       // tensor-core tile kernel (pinn_wide_kernel.cuh)
     int maxt;                                // threads per CTA the step kernels are compiled for
-    StepKernelFn wide128;                    // the tile kernel's class for hidden widths up to 128, 512 threads
+    StepKernelFn wide128;                    // the tile kernel's class for hidden widths up to 128
+    // networks of 2..4 outputs (order 2, at most four directions; null elsewhere):
+    StepKernelFn coupled[2];                 // coupled_step_kernel [GMEM]
+    StepKernelFn coupled_wide128;            // the coupled form of the 128-wide tile kernel
 };
-
-// The step kernels of one jet set for networks of 2..4 outputs: coupled_step_kernel [GMEM], and the coupled form of the
-// 128-wide tile kernel.  Their own table, filled by the 'coupled' and 'wide128_coupled' build units;
-// coupled_kernels(nf, ns) is nullptr outside 0 <= ns <= nf <= 4.
-struct CoupledSet {
-    StepKernelFn step[2];
-    StepKernelFn wide128;                    // wide128_coupled_step_kernel (pinn_wide_kernel.cuh), 512 threads
-};
-const CoupledSet* coupled_kernels(int nf, int ns);
-CoupledSet& coupled_slot(int nf, int ns);
 
 // The set of a jet set, or nullptr when none was built: 0 <= ns <= nf <= PINN_MAX_DIRS for order 2; 1 <= nf <= 4 and
 // ns = 0 for orders 3 / 4 (their plans carry no second-order channels).  Defined in pinn_kernels.cu.

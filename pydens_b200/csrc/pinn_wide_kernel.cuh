@@ -9,7 +9,7 @@
 // networks whose weights the thread kernel cannot hold in shared memory); the tile is T = 8192 / KW points.
 //
 //   * CTA tile = T collocation points (128 or 64); 512 threads: thread (p, part) owns point p and 16 of the KW hidden
-//     units, so every per-(point, unit) quantity is thread-private (KW = 64 at 256 threads: 32 units each).
+//     units, so every per-(point, unit) quantity is thread-private.
 //   * Every hidden->hidden product, for every jet channel c, is one GEMM  Z_c[T x KW] = A_c[T x KW] . W^T
 //     with A_c written row-per-thread into shared memory, W staged [n][k] in shared memory (one layer at a time), and
 //     Z_c written back to shared memory, where the thread of each point reads its row.  The 16 x 32 blocks (16 of them
@@ -44,7 +44,7 @@
 namespace pinn {
 namespace wide {
 
-constexpr int NT_MAX = 512;            // threads per CTA (template NT = 256 or 512): thread = (point, 1/NH of the hidden units)
+constexpr int NT = 512;                // threads per CTA: thread = (point, 1/NH of the hidden units)
 constexpr int MAX_LAYERS = 6;          // linear layers (hidden levels H <= 5, hidden->hidden layers <= 4)
 constexpr int TILE_FLOATS = 8192;      // points per tile x padded width: the same for both width classes
 
@@ -94,7 +94,7 @@ struct Tile {
     static constexpr int M_WOUT = M_WD + PINN_MAX_DIRS * KW;   // output layer weights [KMAX j][KW]
     static constexpr int M_SCAL = M_WOUT + KMAX * KW;          // per warp: loss, sbar, bout[KMAX], vbar[4]  (SCS floats each)
     static constexpr int SCS = MULTI ? 16 : 8;
-    static constexpr int M_END = M_SCAL + SCS * (NT_MAX / 32);
+    static constexpr int M_END = M_SCAL + SCS * (NT / 32);
 
     static_assert(KW == 64 || KW == 128, "width classes");
     static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one CTA");
@@ -307,7 +307,7 @@ __device__ __forceinline__ void gemm_small(uint8_t* smem, float* acc_s, int n, i
 // ansatz is applied per component with the shared boundary factor and time gate, the residual program finds channel c
 // of component j in slot j*C + c and leaves its partial in slot eq_out[1] + j*C + c; the forward-only form writes
 // u [n, k] row-major.
-template <int NF, int NS, int NT, int KW, bool FWD, bool MULTI = false>
+template <int NF, int NS, int KW, bool FWD, bool MULTI = false>
 __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
     using G = Tile<KW, MULTI>;
     constexpr int T = G::T, LDS = G::LDS, LXB = G::LXB;
@@ -328,8 +328,6 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
     float* const wacc_base = G::WACC_SMEM ? reinterpret_cast<float*>(smem + G::S_WACC)
                                           : a.wacc + (size_t)blockIdx.x * G::WACC_FLOATS;
 
-    pdl_wait();                                    // the previous step (its parameter update) is complete and visible
-    pdl_launch_dependents();
     // ---- one-time setup: constants, zeroed accumulators -----------------------------------------------------------
     for (int i = tid; i < G::MISC_FLOATS; i += NT) misc[i] = 0.0f;
     for (int i = tid; i < 16 * LXB; i += NT) reinterpret_cast<float*>(smem + G::S_XB)[i] = 0.0f;
@@ -913,20 +911,20 @@ __device__ __forceinline__ void wide_step(const DevPlan& P, const StepArgs a) {
     finish_grid(a, n_out_floats);
 }
 
-// hidden widths <= 64: 128-point tiles, NT = 512 (four threads per point) or 256 (two)
-template <int NF, int NS, int NT>
-__global__ void __launch_bounds__(NT, 1) wide_step_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
-    wide_step<NF, NS, NT, 64, false>(P, a);
+// hidden widths <= 64: 128-point tiles, four threads per point
+template <int NF, int NS>
+__global__ void __launch_bounds__(512, 1) wide_step_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
+    wide_step<NF, NS, 64, false>(P, a);
 }
 // hidden widths <= 128: 64-point tiles, eight threads per point
 template <int NF, int NS>
 __global__ void __launch_bounds__(512, 1) wide128_step_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
-    wide_step<NF, NS, 512, 128, false>(P, a);
+    wide_step<NF, NS, 128, false>(P, a);
 }
 // the coupled form (networks of 2..4 outputs) of the 128-wide class
 template <int NF, int NS>
 __global__ void __launch_bounds__(512, 1) wide128_coupled_step_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
-    wide_step<NF, NS, 512, 128, false, true>(P, a);
+    wide_step<NF, NS, 128, false, true>(P, a);
 }
 // pinn_forward of the networks only the 128-wide class holds: u of every point to a.out (coupled: [n, k] row-major)
 __global__ void __launch_bounds__(512, 1) wide128_forward_kernel(const __grid_constant__ DevPlan P, const StepArgs a);

@@ -72,17 +72,18 @@ def test_library_is_sm90a_and_stages_weights_with_tma():
     assert 'LDS.128' in out                                 # broadcast 128-bit weight loads
 
 
-def test_kernel_table_points_at_the_right_kernel_instantiations():
+def test_kernel_table_points_every_entry_at_its_kernel_instantiation():
     """ The kernel instantiations live in many build units that fill one table at load time; its lookup
     pinn::kernels(nf, ns, order) must hand out exactly step_kernel<NF, NS, GMEM, MAXT, 16, GEN> and the
-    multi-step, tile and small-batch kernels of every (NF, NS), the five / six direction kernels and
-    hi_step_kernel<NF, K> of orders 3 / 4, and nothing for keys outside those.  Checked on the host against
-    the exported kernel stubs — no GPU needed. """
+    multi-step, small-batch, tile (64- and 128-wide) and coupled-system kernels of every (NF, NS), the five / six
+    direction kernels and hi_step_kernel<NF, K> of orders 3 / 4, null where a jet set has no such kernel, and nothing
+    for keys outside those.  Checked on the host against the exported kernel stubs — no GPU needed. """
     lib = C.CDLL(_native.LIB_PATH)
 
     class KernelSet(C.Structure):
         _fields_ = [('step', (C.c_void_p * 2) * 2), ('multi', C.c_void_p), ('small', C.c_void_p),
-                    ('wide', C.c_void_p * 2), ('maxt', C.c_int)]
+                    ('wide', C.c_void_p), ('maxt', C.c_int), ('wide128', C.c_void_p),
+                    ('coupled', C.c_void_p * 2), ('coupled_wide128', C.c_void_p)]
 
     kernels = lib._ZN4pinn7kernelsEiii
     kernels.restype = C.POINTER(KernelSet)
@@ -94,6 +95,12 @@ def test_kernel_table_points_at_the_right_kernel_instantiations():
     def step(nf, ns, gmem, maxt, gen):
         return addr('_ZN4pinn11step_kernelILi%dELi%dELb%dELi%dELi16ELb%dEEEvNS_7DevPlanENS_8StepArgsE' % (nf, ns, gmem, maxt, gen))
 
+    def wide(name, nf, ns):
+        return addr('_ZN4pinn4wide%d%sILi%dELi%dEEEvNS_7DevPlanENS_8StepArgsE' % (len(name), name, nf, ns))
+
+    def tile_and_coupled_entries_are_null(k):
+        return (k.wide, k.wide128, k.coupled[0], k.coupled[1], k.coupled_wide128) == (None,) * 5
+
     for nf in range(5):
         for ns in range(nf + 1):
             k = kernels(nf, ns, 2).contents
@@ -103,8 +110,11 @@ def test_kernel_table_points_at_the_right_kernel_instantiations():
                 assert [k.step[gen][0], k.step[gen][1]] == [step(nf, ns, 0, maxt, gen), step(nf, ns, 1, maxt, gen)], (nf, ns, gen)
             assert k.multi == addr('_ZN4pinn17multi_step_kernelILi%dELi%dELi%dELi16EEEvNS_7DevPlanENS_9MultiArgsE' % (nf, ns, maxt))
             assert k.small == addr('_ZN4pinn5small17small_step_kernelILi%dELi%dEEEvNS_7DevPlanENS_9MultiArgsE' % (nf, ns))
-            assert list(k.wide) == [addr('_ZN4pinn4wide16wide_step_kernelILi%dELi%dELi%dEEEvNS_7DevPlanENS_8StepArgsE' % (nf, ns, t))
-                                    for t in (512, 256)], (nf, ns)
+            assert k.wide == wide('wide_step_kernel', nf, ns), (nf, ns)
+            assert k.wide128 == wide('wide128_step_kernel', nf, ns), (nf, ns)
+            assert list(k.coupled) == [addr('_ZN4pinn19coupled_step_kernelILi%dELi%dELb%dELi%dEEEvNS_7DevPlanENS_8StepArgsE'
+                                            % (nf, ns, gmem, maxt)) for gmem in (0, 1)], (nf, ns)
+            assert k.coupled_wide128 == wide('wide128_coupled_step_kernel', nf, ns), (nf, ns)
         for order in (3, 4):
             k = kernels(nf, 0, order)
             if nf == 0:
@@ -113,13 +123,13 @@ def test_kernel_table_points_at_the_right_kernel_instantiations():
             k = k.contents
             assert k.step[1][1] == addr('_ZN4pinn2hi14hi_step_kernelILi%dELi%dEEEvNS_7DevPlanENS_8StepArgsE' % (nf, order))
             assert (k.step[0][0], k.step[0][1], k.step[1][0], k.multi, k.small, k.maxt) == (None, None, None, None, None, 256)
-            assert list(k.wide) == [None, None]
+            assert tile_and_coupled_entries_are_null(k), (nf, order)
             assert not kernels(nf, 1, order)
     for nf in (5, 6):
         k = kernels(nf, nf, 2).contents
         assert k.step[1][1] == step(nf, nf, 1, 256, 1) and k.maxt == 256
         assert (k.step[0][0], k.step[0][1], k.step[1][0], k.multi, k.small) == (None, None, None, None, None)
-        assert list(k.wide) == [None, None]
+        assert tile_and_coupled_entries_are_null(k), nf
         for ns in range(nf):
             assert not kernels(nf, ns, 2)
         assert not kernels(nf, 0, 3) and not kernels(nf, 0, 4)

@@ -1,23 +1,22 @@
-""" The tensor-core tile kernel wide_step_kernel<NF, NS, NT> (pydens_b200/csrc/pinn_wide_kernel.cuh) against the fp64
+""" The tensor-core tile kernel wide_step_kernel<NF, NS> (pydens_b200/csrc/pinn_wide_kernel.cuh) against the fp64
 oracle, at every jet set, width, depth and tile edge it accepts.
 
 The host emulation (tests/emul) never runs this kernel's own code: its 3xTF32 GEMMs, the zero-padding to 64 units,
 the slab layout, the exchange area, the shared-memory accumulators that live across the tiles of a CTA and their
 readout.  So every test here runs it on the GPU, through the bare C ABI (plans built by `N.build_spec`, as
 test_gpu_fuzz.py does), with `PINN_FORCE_KERNEL=wide`, and first asserts from pinn_plan_info that the tile kernel
-is the one that runs, with the jet set and the thread count it asked for.
+is the one that runs, with the jet set it asked for and 512 threads per CTA.
 
 Checked against the fp64 oracle with the tolerances and the cancellation factor of test_gpu_placement.py: the loss,
 the residual, the whole gradient and every tensor of it (each W_l, each b_l including the output bias, log_scale and
 each V), a tensor whose gradient is 1000x below the whole held to 1e-3 of the whole.  The oracle runs once per
 problem over one batch and is cut at each prefix.
-- every (NF, NS) with 0 <= NS <= NF <= 4 (the 15 instantiated jet sets), each at 512 and at 256 threads per CTA
-  (PINN_WIDE_THREADS=256: two threads per point), on networks of 2 to 6 linear layers with hidden widths at the
-  16-column block edges and tanh / sigmoid / identity layers; batches of 1, 127, 128, 129 and 128 * sm_count + 1
-  points (one tile past a full round, so one CTA walks two tiles);
-- seeded random tile-eligible problems: point columns 1-8 (parameter columns too), bc / ic ansatz with ic callables
-  that use V, 0-4 variables, log_scale != 0, and on some seeds the criteria tracer.apply_criterion lowers; odd seeds
-  at 256 threads, and batches up to 128 * sm_count + 1 points;
+- every (NF, NS) with 0 <= NS <= NF <= 4 (the 15 instantiated jet sets), on networks of 2 to 6 linear layers with
+  hidden widths at the 16-column block edges and tanh / sigmoid / identity layers; batches of 1, 127, 128, 129 and
+  128 * sm_count + 1 points (one tile past a full round, so one CTA walks two tiles);
+- 60 seeded random tile-eligible problems: point columns 1-8 (parameter columns too), bc / ic ansatz with ic callables
+  that use V, 0-4 variables, log_scale != 0, and on some seeds the criteria tracer.apply_criterion lowers, and batches
+  up to 128 * sm_count + 1 points;
 - tile and grid edges around 128 * sm_count, and about 40 tiles through one CTA (PINN_WIDE_CTAS=1 / 7): the
   accumulators are zeroed once per launch and summed over every tile of the CTA;
 - bit level: in-kernel sampling equals pinn_sample's points (5 and 8 columns: the second Philox block), and steps
@@ -198,19 +197,15 @@ def _abi_step(spec, params, points, **kw):
         return p.info, loss, res, grads
 
 
-def _tile_plan(spec, threads, monkeypatch):
-    """ A plan forced onto the tile kernel at `threads` per CTA; asserts from pinn_plan_info that this is what runs. """
+def _tile_plan(spec, monkeypatch):
+    """ A plan forced onto the tile kernel; asserts from pinn_plan_info that this is what runs. """
     monkeypatch.setenv('PINN_FORCE_KERNEL', 'wide')
-    if threads == 256:
-        monkeypatch.setenv('PINN_WIDE_THREADS', '256')
-    else:
-        monkeypatch.delenv('PINN_WIDE_THREADS', raising=False)
     p = _Plan(spec)
     info = p.info
     try:
         assert info.tensor_core == 1, 'the tile kernel does not run this plan'
         assert (info.nf, info.ns) == (spec.nf, spec.ns), ((info.nf, info.ns), (spec.nf, spec.ns))
-        assert info.threads_per_cta == threads, (info.threads_per_cta, threads)
+        assert info.threads_per_cta == 512, info.threads_per_cta
     except AssertionError:
         p.__exit__(None, None, None)                 # the caller's `with` never starts: destroy the plan here
         raise
@@ -252,7 +247,7 @@ def _params(cfg, spec):
     return params
 
 
-# ---- 1. every jet set x both thread counts ------------------------------------------------------------------------
+# ---- 1. every jet set ---------------------------------------------------------------------------------------------
 def _icf_a(V):
     return lambda *x: torch.sin(1.5 * x[0]) * V('a', 0.4) + 0.3
 
@@ -300,21 +295,20 @@ JET_SETS = {
 }
 
 
-@pytest.mark.parametrize('threads', [512, 256])
 @pytest.mark.parametrize('jet', list(JET_SETS), ids=lambda j: 'nf%d_ns%d' % j)
-def test_every_jet_set_matches_fp64_oracle(jet, threads, monkeypatch):
+def test_every_jet_set_matches_fp64_oracle(jet, monkeypatch):
     cfg = JET_SETS[jet]
     spec, _ = _spec(cfg)
     assert (spec.nf, spec.ns) == jet, 'the equation traces to (%d, %d)' % (spec.nf, spec.ns)
     params = _params(cfg, spec)
-    with _tile_plan(spec, threads, monkeypatch) as p:
+    with _tile_plan(spec, monkeypatch) as p:
         sm = p.info.sm_count
         cuts = [1, 127, 128, 129, 128 * sm + 1]
         pts = _points(cfg, max(cuts), seed=11)
         ref = _oracle_prefixes(('jet', jet), cfg, params, pts, cuts)
         for n in cuts:
             loss, res, grads, _ = p.step(params, pts[:n])
-            _check('%s threads=%d n=%d' % (_tag(cfg, spec), threads, n), spec, (loss, res, grads), ref[n])
+            _check('%s n=%d' % (_tag(cfg, spec), n), spec, (loss, res, grads), ref[n])
 
 
 # ---- 2. seeded random tile-eligible problems --------------------------------------------------------------------
@@ -380,13 +374,12 @@ def _random_tile_problem(seed):
     cfg['eq_name'] = name
     crit = CRITERIA[(seed // 6) % len(CRITERIA)] if seed % 6 == 5 else None
     n = int(rng.choice([1, 127, 129, 1000, 4097, -1]))     # -1: 128 * sm_count + 1, one CTA walks two tiles
-    threads = 256 if seed % 2 else 512
-    return cfg, crit, n, threads
+    return cfg, crit, n
 
 
-@pytest.mark.parametrize('seed', list(range(40)))
+@pytest.mark.parametrize('seed', list(range(60)))
 def test_random_tile_problem_matches_fp64_oracle(seed, monkeypatch):
-    cfg, crit, n, threads = _random_tile_problem(seed)
+    cfg, crit, n = _random_tile_problem(seed)
     if n < 0:
         n = 128 * torch.cuda.get_device_properties(0).multi_processor_count + 1
     pts = _points(cfg, n, seed=5000 + seed)
@@ -409,12 +402,12 @@ def test_random_tile_problem_matches_fp64_oracle(seed, monkeypatch):
         slack = 1.0 + 1e4 * float(near.mean()) * (1.0 if kind == 'l1' else 1e-5)
     spec, _ = _spec(cfg, key)
     assert spec.nf <= 4 and spec.n_params == params.size
-    with _tile_plan(spec, threads, monkeypatch) as p:
+    with _tile_plan(spec, monkeypatch) as p:
         loss, res, grads, _ = p.step(params, pts, inv_n=inv_n)
     ref = _oracle_prefixes(('random', seed), cfg, params, pts, [n], criterion=module)[n]
     if crit is not None:
         ref = (ref[0], r64, ref[2])               # the kernel's residual is the criterion's sqrt(rho(r) + eps)
-    tag = 'seed %d %s %s criterion=%s threads=%d n=%d' % (seed, cfg['eq_name'], _tag(cfg, spec), crit, threads, n)
+    tag = 'seed %d %s %s criterion=%s n=%d' % (seed, cfg['eq_name'], _tag(cfg, spec), crit, n)
     _check(tag, spec, (loss, res, grads), ref, weight=weight, residual=crit is None, slack=slack)
 
 
@@ -446,7 +439,7 @@ def _edge_oracle(name, p):
 @pytest.mark.parametrize('name', list(EDGE))
 def test_tile_and_grid_edges_match_fp64_oracle(name, monkeypatch):
     spec, _ = _spec(EDGE[name])
-    with _tile_plan(spec, 512, monkeypatch) as p:
+    with _tile_plan(spec, monkeypatch) as p:
         cfg, params, pts, ref = _edge_oracle(name, p)
         for n in _edge_cuts(p.info.sm_count):
             loss, res, grads, _ = p.step(params, pts[:n])
@@ -458,7 +451,7 @@ def test_tile_and_grid_edges_match_fp64_oracle(name, monkeypatch):
 def test_many_tiles_per_cta_match_fp64_oracle(name, ctas, monkeypatch):
     """ PINN_WIDE_CTAS caps the grid: each CTA walks 40 (1 CTA) or 5-6 (7 CTAs) tiles into one set of accumulators """
     spec, _ = _spec(EDGE[name])
-    with _tile_plan(spec, 512, monkeypatch) as p:
+    with _tile_plan(spec, monkeypatch) as p:
         cfg, params, pts, ref = _edge_oracle(name, p)
         monkeypatch.setenv('PINN_WIDE_CTAS', str(ctas))
         n = MANY_TILES
@@ -481,16 +474,15 @@ def _columns(total):
     return base[:total]
 
 
-@pytest.mark.parametrize('threads', [512, 256])
 @pytest.mark.parametrize('total', [5, 8])
-def test_in_kernel_sampling_equals_explicit_points(total, threads, monkeypatch):
+def test_in_kernel_sampling_equals_explicit_points(total, monkeypatch):
     """ columns 4 .. 7 come from the second Philox block; a nonzero point_offset shifts the counter """
     cfg = _sampling_problem(total)
     spec, _ = _spec(cfg)
     params = _params(cfg, spec)
     cols = _columns(total)
     n, seed, step, offset = 3001, 4242, (3 << 32) | 17, 123457
-    with _tile_plan(spec, threads, monkeypatch) as p:
+    with _tile_plan(spec, monkeypatch) as p:
         _, res_s, _, out_s = p.step(params, None, n=n, cols=cols, seed=seed, step=step, offset=offset)
         out_s = out_s.clone()
         pts = p.sample(n, cols, seed, step, offset)
@@ -503,13 +495,13 @@ def test_in_kernel_sampling_equals_explicit_points(total, threads, monkeypatch):
     assert np.array_equal(res_s, res_e)
 
 
-@pytest.mark.parametrize('threads,ctas', [(512, None), (256, None), (512, 1)])
-def test_step_is_bit_reproducible(threads, ctas, monkeypatch):
+@pytest.mark.parametrize('ctas', [None, 1])
+def test_step_is_bit_reproducible(ctas, monkeypatch):
     cfg = EDGE['wide64']
     spec, _ = _spec(cfg)
     params = _params(cfg, spec)
     pts = _points(cfg, 20011 if ctas is None else 3001, seed=31)
-    with _tile_plan(spec, threads, monkeypatch) as p:
+    with _tile_plan(spec, monkeypatch) as p:
         if ctas is not None:
             monkeypatch.setenv('PINN_WIDE_CTAS', str(ctas))
         runs = [p.step(params, pts) for _ in range(3)]
@@ -533,7 +525,6 @@ def _first_second(u, x, y, D, V):               # (2, 1): four jet channels
 def test_default_selection_at_its_boundary(eq, width, tile, monkeypatch):
     """ by default the tile kernel takes networks with a hidden layer of 48 units or more and at least 5 channels """
     monkeypatch.delenv('PINN_FORCE_KERNEL', raising=False)
-    monkeypatch.delenv('PINN_WIDE_THREADS', raising=False)
     cfg = _problem(eq, 2, [(width, 'Tanh'), (16, 'Tanh')], bc=0.0)
     spec, traced = _spec(cfg)
     with _Plan(spec) as p:
@@ -585,7 +576,7 @@ def test_largest_network_the_tile_kernel_claims(monkeypatch):
     spec, _ = _spec(cfg)
     assert spec.n_layers == 6 and spec.n_vars == 4 and spec.ndims + spec.nparams == 8
     params = _params(cfg, spec)
-    with _tile_plan(spec, 512, monkeypatch) as p:
+    with _tile_plan(spec, monkeypatch) as p:
         cuts = [1, 129, 128 * p.info.sm_count + 1]
         pts = _points(cfg, max(cuts), seed=41)
         ref = _oracle_prefixes(('largest',), cfg, params, pts, cuts)

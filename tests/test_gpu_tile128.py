@@ -1,4 +1,4 @@
-""" The 128-wide class of the tensor-core tile kernel, wide_step_kernel<NF, NS, 512, 128> and its forward-only form
+""" The 128-wide class of the tensor-core tile kernel, wide128_step_kernel<NF, NS> and its forward-only form
 (pydens_b200/csrc/pinn_wide_kernel.cuh), against the fp64 oracle and the unmodified reference.
 
 Networks with hidden layers of 65-128 units whose weights do not fit the thread kernel's shared memory (e.g. 3 x 128 or
@@ -43,7 +43,6 @@ def _plan128(spec, monkeypatch, force=True):
         monkeypatch.setenv('PINN_FORCE_KERNEL', 'wide128')
     else:
         monkeypatch.delenv('PINN_FORCE_KERNEL', raising=False)
-    monkeypatch.delenv('PINN_WIDE_THREADS', raising=False)
     p = TG._Plan(spec)
     try:
         assert p.info.tensor_core == 2, 'the 128-wide tile kernel does not run this plan (%d)' % p.info.tensor_core
@@ -213,7 +212,7 @@ def test_every_jet_set_matches_fp64_oracle(jet, monkeypatch):
 def _random_wide_problem(seed):
     """ test_gpu_tile's random problem generator (equation, columns, ansatz, variables, criterion, batch) on hidden
     widths of the 128-wide class: at the block edges or uniform in 1..128, at least one above 64 """
-    cfg, crit, n, _ = TG._random_tile_problem(400 + seed)
+    cfg, crit, n = TG._random_tile_problem(400 + seed)
     rng = np.random.RandomState(520000 + seed)
     hidden = [(int(rng.choice(EDGE_WIDTHS)) if rng.rand() < 0.6 else int(rng.randint(1, 129)), a)
               for _, a in cfg['hidden']]

@@ -73,7 +73,7 @@ def env(**kv):
 
 def _plan(spec, force=True):
     """ A plan on the coupled 128-wide tile kernel (forced, or by default); asserts from pinn_plan_info that it runs. """
-    with env(PINN_FORCE_KERNEL='wide128' if force else None, PINN_WIDE_THREADS=None):
+    with env(PINN_FORCE_KERNEL='wide128' if force else None):
         p = TG._Plan(spec)
     try:
         assert p.info.tensor_core == 2, 'the 128-wide tile kernel does not run this plan (%d)' % p.info.tensor_core
@@ -90,7 +90,7 @@ def _create_rc(spec, force):
     """ pinn_plan_create's return code and plan info under PINN_FORCE_KERNEL=force (None: default selection) """
     lib = N.load()
     plan = C.c_void_p()
-    with env(PINN_FORCE_KERNEL=force, PINN_WIDE_THREADS=None):
+    with env(PINN_FORCE_KERNEL=force):
         rc = lib.pinn_plan_create(C.byref(spec), 0, C.byref(plan))
     info = None
     if rc == 0:
