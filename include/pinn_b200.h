@@ -397,6 +397,36 @@ int pinn_multi_step_terms(const PinnPlan* plan, float* params, float* exp_avg, f
                           float* losses_ring, int64_t ring_len, float point_weight, int n_terms,
                           const PinnTerm* terms, void* stream);
 
+/*
+ * ENSEMBLES of tiny-batch fits in one launch: pinn_multi_step_terms for `n_members` fits of the same plan side by side,
+ * one CTA (multi-step kernel) or one cluster (cluster kernel) per member.  A PinnMember holds what differs between the
+ * fits: their parameters, Adam state, mask, step tensors, step counter, loss ring, explicit batches (or NULL: sample
+ * in-kernel with `cols` from the member's seed) and optimizer step count; everything else — plan, constraint terms,
+ * batch size, k_steps, Adam hyper-parameters, ring_len, point weight — is shared.  Every member's result is bit-identical
+ * to pinn_multi_step_terms on that member alone: the kernel and the cluster size are chosen by the same rule, and the
+ * members never exchange anything.  The arguments are checked as pinn_multi_step_terms checks them, member by member;
+ * n_members outside 1..PINN_MAX_MEMBERS, a null or misaligned (params: 16 bytes) member pointer: PINN_E_INVALID.
+ * The member table travels to the kernel by value: the call allocates nothing and stays stream-ordered and capturable.
+ */
+#define PINN_MAX_MEMBERS 128
+typedef struct PinnMember {
+    float* params;             /* device [n_params] in/out, 16-byte aligned */
+    float* exp_avg;            /* device [n_params] in/out */
+    float* exp_avg_sq;         /* device [n_params] in/out */
+    const float* mask;         /* device [n_params]: 1 = trainable, 0 = frozen */
+    float* step_tensors;       /* device [n_step_tensors] fp32 step counters of the member's optimizer, += k_steps */
+    int32_t n_step_tensors;
+    float opt_step0;           /* optimizer steps the member took before this launch */
+    const float* points;       /* device [k_steps, n_points, ndims+nparams], or NULL: sample in-kernel */
+    uint64_t seed;
+    uint64_t* step_counter;    /* device step number of the member, += k_steps */
+    float* losses_ring;        /* device [ring_len] */
+} PinnMember;
+int pinn_multi_step_ensemble(const PinnPlan* plan, int n_members, const PinnMember* members, int64_t n_points,
+                             int k_steps, float lr, float beta1, float beta2, float eps, float weight_decay,
+                             int64_t ring_len, float point_weight, int n_terms, const PinnTerm* terms,
+                             const PinnColumn* cols, void* stream);
+
 /* Forward only: u = ansatz(net(x)) for explicit points — the work of Solver.predict
  * (model_torch.py:466-487) and of the `_forward` closure handed to constraints (:451-454).
  * u_out [n_points] for a network of one output, [n_points, k] row-major for k outputs. */

@@ -6,6 +6,7 @@ The fit step runs in hand-written sm_90a CUDA (libpinn_b200.so, C ABI in include
 """
 from .model import D, V, TorchModel, ConvBlockModel, current_model
 from .solver import Solver
+from .ensemble import fit_ensemble
 from .sampler import *            # noqa: F401,F403  (NumpySampler, ConstantSampler, Sampler)
 
 __version__ = '1.0.2+b200.1'

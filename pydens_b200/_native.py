@@ -88,12 +88,22 @@ class PinnTerm(C.Structure):
 
 MAX_TERMS, MAX_TERM_POINTS = 4, 32
 
+
+class PinnMember(C.Structure):
+    """ One fit of pinn_multi_step_ensemble: its parameters, Adam state, step tensors, batches, seed, counter and ring. """
+    _fields_ = [('params', C.c_void_p), ('exp_avg', C.c_void_p), ('exp_avg_sq', C.c_void_p), ('mask', C.c_void_p),
+                ('step_tensors', C.c_void_p), ('n_step_tensors', C.c_int32), ('opt_step0', C.c_float),
+                ('points', C.c_void_p), ('seed', C.c_uint64), ('step_counter', C.c_void_p), ('losses_ring', C.c_void_p)]
+
+
+MAX_MEMBERS = 128
+
 EXPORTS = ('pinn_last_error', 'pinn_abi_version', 'pinn_plan_create', 'pinn_plan_destroy',
            'pinn_workspace_bytes', 'pinn_out_floats', 'pinn_step', 'pinn_forward', 'pinn_sample',
            'pinn_record_loss', 'pinn_plan_info', 'pinn_comm_create', 'pinn_comm_connect', 'pinn_comm_destroy',
            'pinn_step_allreduce', 'pinn_comm_status', 'pinn_pipe_create', 'pinn_pipe_destroy', 'pinn_pipe_buffer',
            'pinn_pipe_step', 'pinn_pipe_finish', 'pinn_pipe_wait', 'pinn_pipe_sync', 'pinn_multi_step',
-           'pinn_multi_step_max_points', 'pinn_step_adam', 'pinn_multi_step_terms')
+           'pinn_multi_step_max_points', 'pinn_step_adam', 'pinn_multi_step_terms', 'pinn_multi_step_ensemble')
 
 LIB_PATH = os.environ.get('PYDENS_B200_LIB') or os.path.join(os.path.dirname(os.path.abspath(__file__)), 'libpinn_b200.so')
 _lib = None
@@ -155,6 +165,9 @@ def load():
                                     C.c_void_p, C.c_int64, C.c_void_p]
     lib.pinn_multi_step_terms.argtypes = lib.pinn_multi_step.argtypes[:-1] + [C.c_float, C.c_int, C.POINTER(PinnTerm),
                                                                               C.c_void_p]
+    lib.pinn_multi_step_ensemble.argtypes = [C.c_void_p, C.c_int, C.POINTER(PinnMember), C.c_int64, C.c_int,
+                                             C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int64,
+                                             C.c_float, C.c_int, C.POINTER(PinnTerm), C.POINTER(PinnColumn), C.c_void_p]
     lib.pinn_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                  C.c_size_t, C.c_void_p]
     lib.pinn_sample.argtypes = [C.c_void_p, C.POINTER(PinnColumn), C.c_uint64, C.c_void_p, C.c_uint64,

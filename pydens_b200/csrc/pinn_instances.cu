@@ -5,11 +5,11 @@
 #include <utility>
 
 #define PINN_STEP 1          // step_kernel, plain problems
-#define PINN_STEP_GEN 2      // step_kernel, general problems, and the persistent multi-step kernel
+#define PINN_STEP_GEN 2      // step_kernel, general problems, and the persistent multi-step kernel (both forms)
 #define PINN_STEP_GMEM 3     // five / six directions: the general step_kernel with per-point state in global memory
 #define PINN_HI_JET 4        // hi_step_kernel, derivatives of order 3 / 4
 #define PINN_WIDE 5          // wide_step_kernel, the tensor-core tile kernel
-#define PINN_SMALL 6         // small_step_kernel, the tiny-batch cluster kernel
+#define PINN_SMALL 6         // small_step_kernel, the tiny-batch cluster kernel (both forms)
 #define PINN_WIDE128 7       // wide_step_kernel of the 128-wide class
 #define PINN_COUPLED 8       // coupled_step_kernel, networks of 2..4 outputs
 #define PINN_WIDE128_COUPLED 9   // wide128_coupled_step_kernel, networks of 2..4 outputs on the 128-wide class
@@ -37,7 +37,10 @@ void enter() {
     KernelSet& k = kernel_slot(NF, J, 2);
     k.step[GEN][0] = step_kernel<NF, J, false, Cfg::MAXT, Cfg::JF, GEN>;
     k.step[GEN][1] = step_kernel<NF, J, true, Cfg::MAXT, Cfg::JF, GEN>;
-    if constexpr (GEN) k.multi = multi_step_kernel<NF, J, Cfg::MAXT, Cfg::JF>;
+    if constexpr (GEN) {
+        k.multi = multi_step_kernel<NF, J, Cfg::MAXT, Cfg::JF>;
+        k.multi_ensemble = multi_step_ensemble_kernel<NF, J, Cfg::MAXT, Cfg::JF>;
+    }
     k.maxt = Cfg::MAXT;
 #elif PINN_UNIT == PINN_STEP_GMEM
     // 13 jet channels per unit do not fit shared memory for any network worth the name; the tracer promotes every
@@ -57,6 +60,7 @@ void enter() {
     kernel_slot(NF, J, 2).wide128 = wide::wide128_step_kernel<NF, J>;
 #elif PINN_UNIT == PINN_SMALL
     kernel_slot(NF, J, 2).small = small::small_step_kernel<NF, J>;
+    kernel_slot(NF, J, 2).small_ensemble = small::small_step_ensemble_kernel<NF, J>;
 #elif PINN_UNIT == PINN_COUPLED
     using Cfg = VariantCfg<NF, J>;
     KernelSet& k = kernel_slot(NF, J, 2);

@@ -169,6 +169,7 @@ struct PinnPlan {
     MultiKernelFn fn_multi;                  // persistent multi-step kernel, or nullptr when it does not fit
     int multi_threads, multi_smem;
     MultiKernelFn fn_small;                  // tiny-batch (<= 128 points) variant, or nullptr
+    EnsembleKernelFn fn_multi_ens, fn_small_ens;   // their ensemble forms, or nullptr (same threads, any smem they take)
     int small_smem;
     int multi_budget, small_budget;          // dynamic shared memory the two can take (constraint programs with more slots)
     int wide_ctas;                           // CTAs the tile kernel runs on (<= sm_count)
@@ -287,7 +288,7 @@ static int multi_smem_bytes(const DevPlan& h, int nw, int rows) {
 }
 
 static void place_multi_kernel(PinnPlan* p) {
-    p->fn_multi = nullptr; p->multi_threads = 0; p->multi_smem = 0; p->multi_budget = 0;
+    p->fn_multi = nullptr; p->multi_threads = 0; p->multi_smem = 0; p->multi_budget = 0; p->fn_multi_ens = nullptr;
     const MultiKernelFn f = p->ks->multi;
     if (!f) return;
     cudaFuncAttributes fm;
@@ -303,13 +304,19 @@ static void place_multi_kernel(PinnPlan* p) {
         }
         if (p->fn_multi && allow_max_smem((const void*)f, p->smem_optin) != cudaSuccess) p->fn_multi = nullptr;
     }
+    p->fn_multi_ens = nullptr;
+    const EnsembleKernelFn fe = p->ks->multi_ensemble;
+    if (p->fn_multi && fe && cudaFuncGetAttributes(&fm, (const void*)fe) == cudaSuccess &&
+        max_warps(fm, p->ks->maxt) * 32 >= p->multi_threads && p->smem_optin - (int)fm.sharedSizeBytes - 64 >= p->multi_budget &&
+        allow_max_smem((const void*)fe, p->smem_optin) == cudaSuccess)
+        p->fn_multi_ens = fe;
     (void)cudaGetLastError();
 }
 
 // Tiny batches: the (point, unit)-parallel loop kernel, for plain dense chains whose jets fit shared memory.  Left out
 // when the jet set has none (more than four directions, orders 3 / 4).
 static void place_small_kernel(PinnPlan* p) {
-    p->fn_small = nullptr; p->small_smem = 0; p->small_budget = 0;
+    p->fn_small = nullptr; p->small_smem = 0; p->small_budget = 0; p->fn_small_ens = nullptr;
     const MultiKernelFn f = p->ks->small;
     if (!f) return;
     const DevPlan& h = p->h;
@@ -319,6 +326,10 @@ static void place_small_kernel(PinnPlan* p) {
     if (cudaFuncGetAttributes(&fs, (const void*)f) == cudaSuccess && bytes <= p->smem_optin - (int)fs.sharedSizeBytes - 64 &&
         allow_max_smem((const void*)f, p->smem_optin) == cudaSuccess) {
         p->fn_small = f; p->small_smem = bytes; p->small_budget = p->smem_optin - (int)fs.sharedSizeBytes - 64;
+        const EnsembleKernelFn fe = p->ks->small_ensemble;
+        if (fe && cudaFuncGetAttributes(&fs, (const void*)fe) == cudaSuccess &&
+            p->smem_optin - (int)fs.sharedSizeBytes - 64 >= p->small_budget && allow_max_smem((const void*)fe, p->smem_optin) == cudaSuccess)
+            p->fn_small_ens = fe;
     }
     (void)cudaGetLastError();
 }
@@ -795,21 +806,24 @@ static int term_matches(const PinnPlan* p, const PinnPlan* q, DevTerm& t) {
     return PINN_OK;
 }
 
-extern "C" int pinn_multi_step_terms(const PinnPlan* cp, float* params, float* exp_avg, float* exp_avg_sq, const float* mask,
-                                     float* step_tensors, int n_step_tensors, const float* points, const PinnColumn* cols,
-                                     uint64_t seed, uint64_t* step_counter, int64_t n_points, int k_steps,
-                                     float lr, float beta1, float beta2, float eps, float weight_decay, float opt_step0,
-                                     float* losses_ring, int64_t ring_len, float point_weight, int n_terms,
-                                     const PinnTerm* terms, void* stream) {
-    PinnPlan* p = const_cast<PinnPlan*>(cp);
-    if (!p || !params || !exp_avg || !exp_avg_sq || !mask || !step_counter || !losses_ring)
-        return fail(PINN_E_INVALID, "null argument");
+// What pinn_multi_step_terms and pinn_multi_step_ensemble share: the checks of the shared arguments and the terms, the
+// by-value plan and arguments, and the kernel the columns go to — the cluster kernel at nc CTAs, or the multi-step kernel.
+struct MultiLaunch {
+    DevPlan plan;
+    MultiArgs a;
+    bool small;
+    int nc, smem;
+};
+
+static int multi_setup(PinnPlan* p, int64_t n_points, int k_steps, float lr, float beta1, float beta2, float eps,
+                       float weight_decay, int64_t ring_len, float point_weight, int n_terms, const PinnTerm* terms,
+                       MultiLaunch& L) {
     if (!p->fn_multi && !p->fn_small) return fail(PINN_E_UNSUPPORTED, "the persistent multi-step kernels do not fit this network in shared memory");
     if (n_terms < 0 || n_terms > PINN_MAX_TERMS || (n_terms > 0 && !terms))
         return fail(PINN_E_INVALID, "pinn_multi_step_terms: %d terms (0..%d)", n_terms, PINN_MAX_TERMS);
     if (!(point_weight >= 0.0f) || point_weight > 3.0e38f) return fail(PINN_E_INVALID, "point_weight must be finite and >= 0");
-    MultiArgs a;
-    memset(&a.terms, 0, sizeof(a.terms));
+    MultiArgs& a = L.a;
+    memset(&a, 0, sizeof(a));
     a.terms.n_terms = n_terms;
     int rows = p->h.rows_total, n_slots = p->h.n_slots;             // scratch rows: the most any program needs
     for (int t = 0; t < n_terms; ++t) {
@@ -830,47 +844,109 @@ extern "C" int pinn_multi_step_terms(const PinnPlan* cp, float* params, float* e
     }
     a.terms.first[n_terms] = a.terms.n_points;
     const long long n_cols = n_points + a.terms.n_points;
-    if (n_points <= 0 || n_cols > pinn_multi_step_max_points(p) || k_steps <= 0 || ring_len <= 0 || n_step_tensors < 0)
+    if (n_points <= 0 || n_cols > pinn_multi_step_max_points(p) || k_steps <= 0 || ring_len <= 0)
         return fail(PINN_E_INVALID, "pinn_multi_step: n_points %lld + %d constraint points (1..%d), k_steps %d", (long long)n_points,
                     a.terms.n_points, pinn_multi_step_max_points(p), k_steps);
-    if (!aligned16(params)) return fail(PINN_E_ALIGN, "params must be 16-byte aligned");
-    DevPlan plan = p->h;
-    plan.n_slots = n_slots;                                         // the small kernel's scratch rows
-    if (!points) { int rc = resolve_cols(p, cols, plan.cols); if (rc) return rc; }
-    a.params = params; a.exp_avg = exp_avg; a.exp_avg_sq = exp_avg_sq; a.mask = mask;
-    a.step_tensors = step_tensors; a.n_step_tensors = n_step_tensors; a.points = points; a.seed = seed;
-    a.step_counter = reinterpret_cast<unsigned long long*>(step_counter);
+    L.plan = p->h;
+    L.plan.n_slots = n_slots;                                       // the small kernel's scratch rows
     a.n_points = n_points; a.inv_n = point_weight; a.k_steps = k_steps;
-    a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = weight_decay; a.opt_step0 = opt_step0;
-    a.losses_ring = losses_ring; a.ring_len = ring_len;
+    a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = weight_decay;
+    a.ring_len = ring_len;
     a.rows_total = rows;
     // batches of at most 128 points: the (point, unit)-parallel kernel (PINN_MULTI_KERNEL=tile forces the other one)
     const char* mk = getenv("PINN_MULTI_KERNEL");
-    const bool small_ok = p->fn_small && n_cols <= 8 * pinn::small::BP && (n_cols <= 256 || !p->fn_multi) &&
-                          !(mk && !strcmp(mk, "tile") && p->fn_multi);
-    if (small_ok) {
-        const int smem = n_slots == p->h.n_slots ? p->small_smem : small::make_layout(plan).total * 4;
-        if (smem > p->small_budget) return fail(PINN_E_UNSUPPORTED, "the constraint programs' scratch slots do not fit shared memory");
+    L.small = p->fn_small && n_cols <= 8 * pinn::small::BP && (n_cols <= 256 || !p->fn_multi) &&
+              !(mk && !strcmp(mk, "tile") && p->fn_multi);
+    if (L.small) {
+        L.smem = n_slots == p->h.n_slots ? p->small_smem : small::make_layout(L.plan).total * 4;
+        if (L.smem > p->small_budget) return fail(PINN_E_UNSUPPORTED, "the constraint programs' scratch slots do not fit shared memory");
         // a cluster of up to 8 CTAs (8 SMs) shares the columns, ~16 per CTA at least; PINN_SMALL_CLUSTER overrides
         int nc = (int)((n_cols + 15) / 16);
         if (nc > 8) nc = 8;
         { const char* e = getenv("PINN_SMALL_CLUSTER"); if (e && atoi(e) >= 1 && atoi(e) <= 8) nc = atoi(e); }
         while ((n_cols + nc - 1) / nc > pinn::small::BP) ++nc;
         if (nc == 3) nc = 4; else if (nc > 4 && nc < 8) nc = 8;         // cluster sizes 1, 2, 4, 8
-        cudaLaunchConfig_t cfg;
-        memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = dim3(nc); cfg.blockDim = dim3(pinn::small::NT); cfg.dynamicSmemBytes = smem;
-        cfg.stream = (cudaStream_t)stream;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = nc; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        CUDA_TRY(cudaLaunchKernelEx(&cfg, p->fn_small, plan, a));
+        L.nc = nc;
     } else {
-        const int smem = rows == p->h.rows_total ? p->multi_smem : multi_smem_bytes(p->h, p->multi_threads / 32, rows);
-        if (smem > p->multi_budget) return fail(PINN_E_UNSUPPORTED, "the constraint programs' scratch slots do not fit shared memory");
-        p->fn_multi<<<1, p->multi_threads, smem, (cudaStream_t)stream>>>(plan, a);
+        L.nc = 1;
+        L.smem = rows == p->h.rows_total ? p->multi_smem : multi_smem_bytes(p->h, p->multi_threads / 32, rows);
+        if (L.smem > p->multi_budget) return fail(PINN_E_UNSUPPORTED, "the constraint programs' scratch slots do not fit shared memory");
     }
+    return PINN_OK;
+}
+
+// The cluster kernel on n_members clusters of L.nc CTAs (member c: CTAs c * nc .. c * nc + nc - 1).
+template <class... Args>
+static int launch_clusters(void (*fn)(const DevPlan, const MultiArgs, Args...), const MultiLaunch& L, int n_members,
+                           void* stream, const Args&... extra) {
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3(L.nc * n_members); cfg.blockDim = dim3(pinn::small::NT); cfg.dynamicSmemBytes = L.smem;
+    cfg.stream = (cudaStream_t)stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = L.nc; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    CUDA_TRY(cudaLaunchKernelEx(&cfg, fn, L.plan, L.a, extra...));
+    CUDA_TRY(cudaGetLastError());
+    return PINN_OK;
+}
+
+extern "C" int pinn_multi_step_terms(const PinnPlan* cp, float* params, float* exp_avg, float* exp_avg_sq, const float* mask,
+                                     float* step_tensors, int n_step_tensors, const float* points, const PinnColumn* cols,
+                                     uint64_t seed, uint64_t* step_counter, int64_t n_points, int k_steps,
+                                     float lr, float beta1, float beta2, float eps, float weight_decay, float opt_step0,
+                                     float* losses_ring, int64_t ring_len, float point_weight, int n_terms,
+                                     const PinnTerm* terms, void* stream) {
+    PinnPlan* p = const_cast<PinnPlan*>(cp);
+    if (!p || !params || !exp_avg || !exp_avg_sq || !mask || !step_counter || !losses_ring)
+        return fail(PINN_E_INVALID, "null argument");
+    MultiLaunch L;
+    if (int rc = multi_setup(p, n_points, k_steps, lr, beta1, beta2, eps, weight_decay, ring_len, point_weight, n_terms, terms, L))
+        return rc;
+    if (n_step_tensors < 0) return fail(PINN_E_INVALID, "pinn_multi_step: n_step_tensors %d", n_step_tensors);
+    if (!aligned16(params)) return fail(PINN_E_ALIGN, "params must be 16-byte aligned");
+    if (!points) { int rc = resolve_cols(p, cols, L.plan.cols); if (rc) return rc; }
+    MultiArgs& a = L.a;
+    a.params = params; a.exp_avg = exp_avg; a.exp_avg_sq = exp_avg_sq; a.mask = mask;
+    a.step_tensors = step_tensors; a.n_step_tensors = n_step_tensors; a.points = points; a.seed = seed;
+    a.step_counter = reinterpret_cast<unsigned long long*>(step_counter);
+    a.opt_step0 = opt_step0;
+    a.losses_ring = losses_ring;
+    if (L.small) return launch_clusters(p->fn_small, L, 1, stream);
+    p->fn_multi<<<1, p->multi_threads, L.smem, (cudaStream_t)stream>>>(L.plan, a);
+    CUDA_TRY(cudaGetLastError());
+    return PINN_OK;
+}
+
+extern "C" int pinn_multi_step_ensemble(const PinnPlan* cp, int n_members, const PinnMember* members, int64_t n_points,
+                                        int k_steps, float lr, float beta1, float beta2, float eps, float weight_decay,
+                                        int64_t ring_len, float point_weight, int n_terms, const PinnTerm* terms,
+                                        const PinnColumn* cols, void* stream) {
+    PinnPlan* p = const_cast<PinnPlan*>(cp);
+    if (!p || !members) return fail(PINN_E_INVALID, "null argument");
+    if (n_members < 1 || n_members > PINN_MAX_MEMBERS)
+        return fail(PINN_E_INVALID, "pinn_multi_step_ensemble: %d members (1..%d)", n_members, PINN_MAX_MEMBERS);
+    bool sample = false;
+    for (int j = 0; j < n_members; ++j) {
+        const PinnMember& m = members[j];
+        if (!m.params || !m.exp_avg || !m.exp_avg_sq || !m.mask || !m.step_counter || !m.losses_ring || m.n_step_tensors < 0 ||
+            (m.n_step_tensors > 0 && !m.step_tensors))
+            return fail(PINN_E_INVALID, "member %d: null pointer or n_step_tensors %d", j, m.n_step_tensors);
+        if (!aligned16(m.params)) return fail(PINN_E_INVALID, "member %d: params must be 16-byte aligned", j);
+        if (!m.points) sample = true;
+    }
+    static thread_local MultiLaunch L;                               // 13 KB: off the stack
+    static thread_local DevMembers table;                            // 10 KB
+    if (int rc = multi_setup(p, n_points, k_steps, lr, beta1, beta2, eps, weight_decay, ring_len, point_weight, n_terms, terms, L))
+        return rc;
+    if (L.small ? !p->fn_small_ens : !p->fn_multi_ens)
+        return fail(PINN_E_UNSUPPORTED, "the ensemble form of the persistent kernel does not fit this network");
+    if (sample) { int rc = resolve_cols(p, cols, L.plan.cols); if (rc) return rc; }
+    memset(&table, 0, sizeof(table));
+    memcpy(table.m, members, sizeof(PinnMember) * (size_t)n_members);
+    if (L.small) return launch_clusters(p->fn_small_ens, L, n_members, stream, table);
+    p->fn_multi_ens<<<n_members, p->multi_threads, L.smem, (cudaStream_t)stream>>>(L.plan, L.a, table);
     CUDA_TRY(cudaGetLastError());
     return PINN_OK;
 }

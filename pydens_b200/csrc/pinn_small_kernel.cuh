@@ -62,8 +62,9 @@ __host__ __device__ inline Layout make_layout(const DevPlan& P) {
     return L;
 }
 
-template <int NF, int NS>
-__global__ void __launch_bounds__(NT, 1) small_step_kernel(const __grid_constant__ DevPlan P, const __grid_constant__ MultiArgs a) {
+// The body of both forms: the fields of `mb` (MultiArgs itself, or one row of the member table) are the fit's own state.
+template <int NF, int NS, class MB>
+__device__ __forceinline__ void small_step_body(const DevPlan& P, const MultiArgs& a, const MB& mb) {
     constexpr int C = 1 + NF + NS;
     extern __shared__ __align__(16) float smem[];
     const int tid = threadIdx.x, lane = tid & 31;
@@ -90,8 +91,8 @@ __global__ void __launch_bounds__(NT, 1) small_step_kernel(const __grid_constant
     while ((1 << ps_log) < Bp) ++ps_log;
     const int PS = 1 << ps_log;
 
-    for (int i = tid; i < P.n_params; i += NT) { flat[i] = a.params[i]; mom1[i] = a.exp_avg[i]; mom2[i] = a.exp_avg_sq[i]; }
-    const unsigned long long step0 = *a.step_counter;
+    for (int i = tid; i < P.n_params; i += NT) { flat[i] = mb.params[i]; mom1[i] = mb.exp_avg[i]; mom2[i] = mb.exp_avg_sq[i]; }
+    const unsigned long long step0 = *mb.step_counter;
     __syncthreads();
 
     for (int s = 0; s < a.k_steps; ++s) {
@@ -101,17 +102,17 @@ __global__ void __launch_bounds__(NT, 1) small_step_kernel(const __grid_constant
             const int p = tid, pe = base + (p < B ? p : B - 1);
             if (pe >= a.n_points) {                                      // a constraint point: fixed, no sampler draw
                 for (int k = 0; k < P.total; ++k) X[k * SR + p] = a.terms.x[pe - a.n_points][k];
-            } else if (a.points) {
-                const float* src = a.points + ((size_t)s * a.n_points + (size_t)pe) * P.total;
+            } else if (mb.points) {
+                const float* src = mb.points + ((size_t)s * a.n_points + (size_t)pe) * P.total;
                 for (int k = 0; k < P.total; ++k) X[k * SR + p] = __ldg(src + k);
             } else {
                 const uint64_t gidx = (uint64_t)pe;
                 const uint32_t c3 = (uint32_t)(((step >> 32) & 0xffffu) << 16);
-                Philox4 b0 = philox4x32_10((uint32_t)gidx, (uint32_t)(gidx >> 32), (uint32_t)step, c3, (uint32_t)a.seed, (uint32_t)(a.seed >> 32));
+                Philox4 b0 = philox4x32_10((uint32_t)gidx, (uint32_t)(gidx >> 32), (uint32_t)step, c3, (uint32_t)mb.seed, (uint32_t)(mb.seed >> 32));
                 Philox4 b1 = b0;
                 if (P.total > 4)
-                    b1 = philox4x32_10((uint32_t)gidx, (uint32_t)(gidx >> 32), (uint32_t)step, c3 | 1u, (uint32_t)a.seed, (uint32_t)(a.seed >> 32));
-                for (int k = 0; k < P.total; ++k) X[k * SR + p] = sample_column(P.cols[k], k, gidx, step, a.seed, b0, b1);
+                    b1 = philox4x32_10((uint32_t)gidx, (uint32_t)(gidx >> 32), (uint32_t)step, c3 | 1u, (uint32_t)mb.seed, (uint32_t)(mb.seed >> 32));
+                for (int k = 0; k < P.total; ++k) X[k * SR + p] = sample_column(P.cols[k], k, gidx, step, mb.seed, b0, b1);
             }
         }
         // the partial gradient alternates between two buffers: a CTA that runs ahead into step s+1 never touches the
@@ -119,7 +120,7 @@ __global__ void __launch_bounds__(NT, 1) small_step_kernel(const __grid_constant
         float* g = smem + Y.g + (s & 1) * g_stride;
         for (int i = tid; i < n_out_floats; i += NT) g[i] = 0.0f;
         // Adam's bias corrections do not depend on the gradient: computed here, off the critical path
-        const float t_opt = a.opt_step0 + (float)(s + 1);
+        const float t_opt = mb.opt_step0 + (float)(s + 1);
         const float bc1 = 1.0f - powf(a.beta1, t_opt);
         const float bc2_sqrt = sqrtf(1.0f - powf(a.beta2, t_opt));
         const float step_size = a.lr / bc1;
@@ -336,7 +337,7 @@ __global__ void __launch_bounds__(NT, 1) small_step_kernel(const __grid_constant
         // ---- Adam (torch.optim.Adam, fused form) on the flat copy ------------------------------------------------------
         {
             for (int i = tid; i < P.n_params; i += NT) {
-                if (a.mask[i] != 0.0f) {
+                if (mb.mask[i] != 0.0f) {
                     float gi = gsum[i];
                     const float pv = flat[i];
                     if (a.weight_decay != 0.0f) gi = fmaf(a.weight_decay, pv, gi);
@@ -346,17 +347,31 @@ __global__ void __launch_bounds__(NT, 1) small_step_kernel(const __grid_constant
                     mom1[i] = m1; mom2[i] = m2;
                 }
             }
-            if (tid == 0 && crank == 0) a.losses_ring[(step0 + (unsigned long long)s) % (unsigned long long)a.ring_len] = gsum[P.n_params];
+            if (tid == 0 && crank == 0) mb.losses_ring[(step0 + (unsigned long long)s) % (unsigned long long)a.ring_len] = gsum[P.n_params];
         }
         __syncthreads();
     }
     if (csize > 1) cluster.sync();                               // every CTA has read the step counter before rank 0 advances it
     if (crank == 0) {                                            // the replicas are bit-identical: rank 0 writes them back
-        for (int i = tid; i < P.n_params; i += NT) { a.params[i] = flat[i]; a.exp_avg[i] = mom1[i]; a.exp_avg_sq[i] = mom2[i]; }
-        for (int i = tid; i < a.n_step_tensors; i += NT) a.step_tensors[i] += (float)a.k_steps;
-        if (tid == 0) *a.step_counter = step0 + (unsigned long long)a.k_steps;
+        for (int i = tid; i < P.n_params; i += NT) { mb.params[i] = flat[i]; mb.exp_avg[i] = mom1[i]; mb.exp_avg_sq[i] = mom2[i]; }
+        for (int i = tid; i < mb.n_step_tensors; i += NT) mb.step_tensors[i] += (float)a.k_steps;
+        if (tid == 0) *mb.step_counter = step0 + (unsigned long long)a.k_steps;
     }
     (void)lane;
+}
+
+template <int NF, int NS>
+__global__ void __launch_bounds__(NT, 1) small_step_kernel(const __grid_constant__ DevPlan P, const __grid_constant__ MultiArgs a) {
+    small_step_body<NF, NS>(P, a, a);
+}
+
+// The ensemble form (pinn_multi_step_ensemble): cluster c trains member c of the table.  Its CTAs exchange their
+// partials with each other only, in rank order, so each member's steps are those of its solo launch at the same
+// cluster size.
+template <int NF, int NS>
+__global__ void __launch_bounds__(NT, 1) small_step_ensemble_kernel(const __grid_constant__ DevPlan P, const __grid_constant__ MultiArgs a,
+                                                                    const __grid_constant__ DevMembers m) {
+    small_step_body<NF, NS>(P, a, m.m[blockIdx.x / cg::this_cluster().num_blocks()]);
 }
 
 }  // namespace small

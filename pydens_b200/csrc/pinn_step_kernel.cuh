@@ -557,9 +557,17 @@ struct MultiArgs {
 };
 // kernel parameters are limited to 32764 bytes (CUDA 12.1+ on Hopper); 16 bytes for the alignment of the second one
 static_assert(sizeof(DevPlan) + sizeof(MultiArgs) + 16 <= 32764, "DevPlan + MultiArgs exceed the kernel-parameter limit");
+// The member table of the ensemble form: what differs between the fits of an ensemble (the MultiArgs fields of the same
+// names are unused there).  A third __grid_constant__ parameter, read in place by the member's CTAs.
+struct DevMembers {
+    PinnMember m[PINN_MAX_MEMBERS];
+};
+static_assert(sizeof(DevPlan) + sizeof(MultiArgs) + sizeof(DevMembers) + 32 <= 32764,
+              "DevPlan + MultiArgs + the member table exceed the kernel-parameter limit");
 
-template <int NF, int NS, int MAXT, int JF>
-__global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_constant__ DevPlan P, const __grid_constant__ MultiArgs a) {
+// The body of both forms: the fields of `mb` (MultiArgs itself, or one row of the member table) are the fit's own state.
+template <int NF, int NS, int JF, class MB>
+__device__ __forceinline__ void multi_step_body(const DevPlan& P, const MultiArgs& a, const MB& mb) {
     extern __shared__ __align__(16) float smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
     const int n_out_floats = P.n_params + 4;
@@ -570,11 +578,11 @@ __global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_consta
     float* mom1 = flat + align4(P.n_params);
     float* mom2 = mom1 + align4(P.n_params);
     float* gsum = mom2 + align4(P.n_params);
-    stage_weights(smem, SL, P, a.params);
+    stage_weights(smem, SL, P, mb.params);
     float* sw = smem + SL.weights_f;
     float* wacc_all = smem + SL.wacc_f;
     for (int i = tid; i < P.n_params; i += blockDim.x) {
-        flat[i] = a.params[i]; mom1[i] = a.exp_avg[i]; mom2[i] = a.exp_avg_sq[i];
+        flat[i] = mb.params[i]; mom1[i] = mb.exp_avg[i]; mom2[i] = mb.exp_avg_sq[i];
     }
     __syncthreads();
 
@@ -582,7 +590,7 @@ __global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_consta
     sink.wacc = wacc_all + warp * n_out_floats;
     sink.dump = P.n_params + 2;
     float* st = smem + SL.storage_f + (size_t)warp * a.rows_total * RS + lane;
-    const unsigned long long step0 = *a.step_counter;
+    const unsigned long long step0 = *mb.step_counter;
     const long long n_tiles = (a.n_points + 31) / 32;
 
     for (int s = 0; s < a.k_steps; ++s) {
@@ -602,15 +610,15 @@ __global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_consta
                 const long long pl = tile * 32 + lane;
                 valid = pl < a.n_points;
                 const long long pe = valid ? pl : a.n_points - 1;
-                if (a.points) {
-                    const float* src = a.points + ((size_t)s * a.n_points + (size_t)pe) * P.total;
+                if (mb.points) {
+                    const float* src = mb.points + ((size_t)s * a.n_points + (size_t)pe) * P.total;
                     for (int k = 0; k < P.total; ++k) st[k * RS] = __ldg(src + k);
                 } else {
                     const uint64_t gidx = (uint64_t)pe;
-                    Philox4 b0 = philox_block(gidx, step, a.seed, 0u);
+                    Philox4 b0 = philox_block(gidx, step, mb.seed, 0u);
                     Philox4 b1 = b0;
-                    if (P.total > 4) b1 = philox_block(gidx, step, a.seed, 1u);
-                    for (int k = 0; k < P.total; ++k) st[k * RS] = sample_column(P.cols[k], k, gidx, step, a.seed, b0, b1);
+                    if (P.total > 4) b1 = philox_block(gidx, step, mb.seed, 1u);
+                    for (int k = 0; k < P.total; ++k) st[k * RS] = sample_column(P.cols[k], k, gidx, step, mb.seed, b0, b1);
                 }
             } else {
                 valid = lane < a.terms.n_points;
@@ -635,7 +643,7 @@ __global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_consta
         }
         __syncthreads();
         // fold the warps in warp order, then Adam on the flat copy
-        const float t_opt = a.opt_step0 + (float)(s + 1);
+        const float t_opt = mb.opt_step0 + (float)(s + 1);
         const float bc1 = 1.0f - powf(a.beta1, t_opt);
         const float bc2_sqrt = sqrtf(1.0f - powf(a.beta2, t_opt));
         const float step_size = a.lr / bc1;
@@ -643,7 +651,7 @@ __global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_consta
             float g = 0.0f;
             for (int w = 0; w < nwarps; ++w) g += wacc_all[w * n_out_floats + i];
             gsum[i] = g;
-            if (i < P.n_params && a.mask[i] != 0.0f) {
+            if (i < P.n_params && mb.mask[i] != 0.0f) {
                 float pv = flat[i];
                 if (a.weight_decay != 0.0f) g = fmaf(a.weight_decay, pv, g);
                 const float m1 = fmaf(1.0f - a.beta1, g - mom1[i], mom1[i]);
@@ -654,7 +662,7 @@ __global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_consta
             }
         }
         __syncthreads();
-        if (tid == 0) a.losses_ring[(step0 + (unsigned long long)s) % (unsigned long long)a.ring_len] = gsum[P.n_params];
+        if (tid == 0) mb.losses_ring[(step0 + (unsigned long long)s) % (unsigned long long)a.ring_len] = gsum[P.n_params];
         // the new parameters in both weight layouts (what stage_weights does after its TMA copy)
         for (int l = 0; l < P.n_layers; ++l) {
             const DevLayer& L = P.layer[l];
@@ -670,13 +678,27 @@ __global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_consta
         __syncthreads();
     }
     for (int i = tid; i < P.n_params; i += blockDim.x) {
-        a.params[i] = flat[i]; a.exp_avg[i] = mom1[i]; a.exp_avg_sq[i] = mom2[i];
+        mb.params[i] = flat[i]; mb.exp_avg[i] = mom1[i]; mb.exp_avg_sq[i] = mom2[i];
     }
-    for (int i = tid; i < a.n_step_tensors; i += blockDim.x) a.step_tensors[i] += (float)a.k_steps;
-    if (tid == 0) *a.step_counter = step0 + (unsigned long long)a.k_steps;
+    for (int i = tid; i < mb.n_step_tensors; i += blockDim.x) mb.step_tensors[i] += (float)a.k_steps;
+    if (tid == 0) *mb.step_counter = step0 + (unsigned long long)a.k_steps;
+}
+
+template <int NF, int NS, int MAXT, int JF>
+__global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_constant__ DevPlan P, const __grid_constant__ MultiArgs a) {
+    multi_step_body<NF, NS, JF>(P, a, a);
+}
+
+// The ensemble form (pinn_multi_step_ensemble): CTA b trains member b of the table, with the plan, the terms and the
+// Adam hyper-parameters of `a`; the members share nothing, so each one's steps are those of its solo launch.
+template <int NF, int NS, int MAXT, int JF>
+__global__ void __launch_bounds__(MAXT, 1) multi_step_ensemble_kernel(const __grid_constant__ DevPlan P, const __grid_constant__ MultiArgs a,
+                                                                      const __grid_constant__ DevMembers m) {
+    multi_step_body<NF, NS, JF>(P, a, m.m[blockIdx.x]);
 }
 
 typedef void (*MultiKernelFn)(const DevPlan, const MultiArgs);
+typedef void (*EnsembleKernelFn)(const DevPlan, const MultiArgs, const DevMembers);
 
 typedef void (*StepKernelFn)(const DevPlan, const StepArgs);
 
@@ -695,6 +717,8 @@ struct KernelSet {
     // networks of 2..4 outputs (order 2, at most four directions; null elsewhere):
     StepKernelFn coupled[2];                 // coupled_step_kernel [GMEM]
     StepKernelFn coupled_wide128;            // the coupled form of the 128-wide tile kernel
+    EnsembleKernelFn multi_ensemble;         // the ensemble forms of `multi` and `small` (null where those are)
+    EnsembleKernelFn small_ensemble;
 };
 
 // The set of a jet set, or nullptr when none was built: 0 <= ns <= nf <= PINN_MAX_DIRS for order 2; 1 <= nf <= 4 and

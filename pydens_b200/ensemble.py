@@ -1,0 +1,243 @@
+""" `fit_ensemble` — train several Solvers of one problem side by side in the persistent multi-step kernels.
+
+People who fit small problems rarely fit just one: they run several seeds, sweep the initial value of a `V(...)`
+variable, or solve one equation for many values of a frozen coefficient.  Each such fit alone runs on one CTA or one
+cluster of at most 8 CTAs; `fit_ensemble` puts up to PINN_MAX_MEMBERS of them into one launch
+(pinn_multi_step_ensemble), one CTA or cluster per member.  It means exactly "call `s.fit(...)` on every solver": every
+member keeps its own seed, optimizer state, frozen mask, loss list and step counter, and its result is bit-identical to
+its solo fit.
+"""
+import ctypes as C
+import os
+import warnings
+
+import numpy as np
+import torch
+from torch import nn
+
+from . import _native
+from .engine import _AUTO_PERSISTENT_MIN_ITERS, _AUTO_PERSISTENT_STEPS, _dist
+
+# what each part of the problem's spec describes, for the error that names the difference between two members
+_SPEC_PARTS = (
+    ('network', ('n_layers', 'widths', 'act', 'skip_src', 'w_off', 'b_off', 'n_params', 'log_scale_off')),
+    ('domain', ('ndims', 'nparams', 'dom_lo', 'dom_hi')),
+    ('ansatz', ('has_bc', 'has_ic', 'bc_value', 'n_ic', 'ic_prog', 'ic_out', 'ic_has_vars')),
+    ('equation program', ('abi_version', 'order', 'nf', 'ns', 'dir_col', 'dir_vec', 'n_eq', 'eq_prog', 'eq_out',
+                          'n_slots', 'n_vars', 'var_off')),
+)
+
+
+def spec_difference(a, b):
+    """ None when the two PinnSpecs are byte-identical, else the part that differs: 'network (widths)', ... """
+    raw_a, raw_b = bytes(a), bytes(b)
+    if raw_a == raw_b:
+        return None
+    for part, fields in _SPEC_PARTS:
+        for name in fields:
+            f = getattr(_native.PinnSpec, name)
+            if raw_a[f.offset:f.offset + f.size] != raw_b[f.offset:f.offset + f.size]:
+                return '%s (%s)' % (part, name)
+    return 'spec padding'
+
+
+def check_members(solvers):
+    """ The solvers of an ensemble: at least one, each once, all on one device.  Raises ValueError. """
+    if not solvers:
+        raise ValueError('fit_ensemble: no solvers')
+    seen = {}
+    for j, s in enumerate(solvers):
+        if id(s) in seen:
+            raise ValueError('fit_ensemble: solvers %d and %d are the same Solver' % (seen[id(s)], j))
+        seen[id(s)] = j
+        if s.device != solvers[0].device:
+            raise ValueError('fit_ensemble: solver %d is on %s, solver 0 on %s' % (j, s.device, solvers[0].device))
+
+
+def member_samplers(sampler, n):
+    """ One sampler per member: a list of n samplers, or the one sampler shared by all. """
+    if isinstance(sampler, (list, tuple)):
+        if len(sampler) != n:
+            raise ValueError('fit_ensemble: %d samplers for %d solvers' % (len(sampler), n))
+        return list(sampler)
+    return [sampler] * n
+
+
+def _device_columns(sampler, total):
+    """ The in-kernel columns of a sampler as `_fit_persistent` takes them, or None: sampled on the host. """
+    if sampler is None:
+        return 'uniform', None
+    dev_cols = sampler.device_columns() if hasattr(sampler, 'device_columns') else None
+    if dev_cols is not None and len(dev_cols) == total and os.environ.get('PYDENS_B200_HOST_SAMPLER') != '1':
+        try:
+            cols = _native.make_columns(dev_cols, total)
+            return bytes(cols), cols
+        except ValueError:
+            pass
+    return None, None
+
+
+def fit_ensemble(solvers, niters, batch_size, sampler=None, loss_terms='equation', optimizer='Adam',
+                 criterion=nn.MSELoss(), lr=0.005, steps_per_launch=None, **kwargs):
+    """ `s.fit(niters, batch_size, sampler, loss_terms, optimizer, criterion, lr, ...)` for every solver in `solvers`,
+    in one persistent launch per `steps_per_launch` steps for all of them when each fit is one that `Solver.fit` sends
+    to the persistent multi-step kernels by itself (or with steps_per_launch): plain Adam, one device, the equation
+    term, fused constraints, a batch the kernels take.  The solvers must share the problem byte for byte (equation,
+    network, domain, ansatz, constraints); they differ in their parameters, seeds, optimizer states and frozen masks.
+
+    sampler   None, one sampler shared by all members, or a list with one per member.  In-kernel samplers draw each
+              member's batch from its own seed; a shared host sampler gives each member its batches in member order,
+              launch by launch.
+    Anything the persistent path cannot take fits the solvers one after another with their own `fit`, after one
+    UserWarning giving the reason.  Raises ValueError for the same Solver twice, solvers on different devices, or
+    solvers whose problems differ.
+    """
+    solvers = list(solvers)
+    check_members(solvers)
+    samplers = member_samplers(sampler, len(solvers))
+    loss_terms = tuple(loss_terms) if isinstance(loss_terms, (tuple, list)) else (loss_terms,)
+    why = None
+    if niters > 0:
+        why = _fit_together(solvers, niters, batch_size, samplers, loss_terms, optimizer, criterion, lr,
+                            steps_per_launch, kwargs)
+        if why is None:
+            return
+        warnings.warn('pydens_b200.fit_ensemble: fitting the solvers one after another (%s)' % why, UserWarning,
+                      stacklevel=2)
+    if steps_per_launch is not None:
+        kwargs['steps_per_launch'] = steps_per_launch
+    for s, smp in zip(solvers, samplers):
+        s.fit(niters, batch_size, smp, list(loss_terms), optimizer, criterion, lr, **dict(kwargs))
+
+
+def _fit_together(solvers, niters, batch_size, samplers, loss_terms, optimizer, criterion, lr, steps_per_launch, kwargs):
+    """ The ensemble fit, or the reason it cannot run (nothing has been trained then). """
+    if _dist() is not None:
+        return 'torch.distributed runs several ranks'
+    engines = []
+    for j, s in enumerate(solvers):
+        ok, why = s._fused_possible(criterion, loss_terms)
+        if not ok:
+            return 'solver %d: %s' % (j, why)
+        eng = s._get_engine()
+        if eng is None:
+            return 'solver %d: %s' % (j, s._lower_error)
+        engines.append(eng)
+    for j, eng in enumerate(engines[1:], 1):
+        diff = spec_difference(engines[0].spec, eng.spec)
+        if diff is not None:
+            raise ValueError('fit_ensemble: solver %d differs from solver 0 in its %s' % (j, diff))
+    e0 = engines[0]
+    k = int(steps_per_launch or 0)
+    if k <= 0:                                            # the rule of FusedEngine.fit for tiny batches
+        if not (niters >= _AUTO_PERSISTENT_MIN_ITERS and 0 < batch_size <= int(e0.info.small_batch_points)
+                and os.environ.get('PYDENS_B200_AUTO_PERSISTENT', '1') != '0' and os.environ.get('PYDENS_B200_NO_GRAPH') != '1'):
+            return ('a solo fit of batch %d x %d steps does not take the persistent kernels by itself '
+                    '(pass steps_per_launch)' % (batch_size, niters))
+        k = _AUTO_PERSISTENT_STEPS
+    if batch_size <= 0:
+        return 'batch_size %d' % batch_size
+    terms = [eng._persistent_terms(loss_terms, batch_size) for eng in engines]
+    if any(t is None for t in terms):
+        return ('the constraints do not all run fused (at most %d, with %d points in all), or batch + constraint points '
+                'exceed %d' % (_native.MAX_TERMS, _native.MAX_TERM_POINTS, e0.lib.pinn_multi_step_max_points(e0.plan)))
+    for j, t in enumerate(terms[1:], 1):
+        for i, (a, b) in enumerate(zip(terms[0], t)):
+            diff = spec_difference(a['spec'], b['spec'])
+            if diff is None and a['host_points'].numpy().tobytes() != b['host_points'].numpy().tobytes():
+                diff = 'points'
+            if diff is not None:
+                raise ValueError('fit_ensemble: solver %d differs from solver 0 in constraint %d: %s' % (j, i, diff))
+    total = solvers[0].model.total
+    keys = [_device_columns(smp, total) for smp in samplers]
+    if len({key for key, _ in keys}) > 1:
+        return 'the members\' samplers differ in their in-kernel columns, or some sample on the host'
+    cols = keys[0][1]
+    host = keys[0][0] is None
+    opts = []
+    for eng in engines:
+        opt, _ = eng._optimizer_for(optimizer, lr, dict(kwargs))
+        g = opt.param_groups[0] if opt.param_groups else {}
+        if not (type(opt) is torch.optim.Adam and len(opt.param_groups) == 1 and not g.get('amsgrad')
+                and not g.get('maximize') and not torch.is_tensor(g.get('lr'))):
+            return 'the optimizer is not plain torch.optim.Adam with one parameter group'
+        opts.append(opt)
+    hyper = [(float(o.param_groups[0]['lr']), tuple(map(float, o.param_groups[0]['betas'])),
+              float(o.param_groups[0]['eps']), float(o.param_groups[0]['weight_decay'])) for o in opts]
+    if len(set(hyper)) > 1:
+        return 'the members\' Adam hyper-parameters differ'
+    return _run(solvers, engines, opts, terms[0], niters, batch_size, samplers if host else None, cols, k, hyper[0])
+
+
+def _run(solvers, engines, opts, terms, niters, batch_size, host_samplers, cols, k, hyper):
+    """ `niters` steps of every member, `k` per launch, members in launches of at most MAX_MEMBERS.  Returns None, or
+    the reason the kernels refused the first launch (nothing has been trained then). """
+    lr, (b1, b2), eps, wd = hyper
+    e0 = engines[0]
+    lib, total = e0.lib, solvers[0].model.total
+    total_sum = e0._sum_reduction()
+    term_arr = (_native.PinnTerm * max(1, len(terms)))()
+    for i, e in enumerate(terms):
+        term_arr[i].plan = e['plan'].value
+        term_arr[i].n_points = e['n']
+        term_arr[i].point_weight = 1.0 if total_sum else 1.0 / e['n']
+        term_arr[i].points = e['host_points'].data_ptr()
+    point_weight = 1.0 if total_sum else 1.0 / batch_size
+    M = len(solvers)
+    members = (_native.PinnMember * M)()
+    starts, step0 = [], []
+    for j, (s, eng, opt) in enumerate(zip(solvers, engines, opts)):
+        if s.optimizer is not eng._opt_obj:
+            eng._drop_graphs()
+            eng._opt_obj, eng._opt_key = s.optimizer, None
+        mask = eng._bind_adam_state(opt)
+        m, v, steps, _ = eng._adam_flat
+        mb = members[j]
+        mb.params, mb.exp_avg, mb.exp_avg_sq, mb.mask = eng.flat.data_ptr(), m.data_ptr(), v.data_ptr(), mask.data_ptr()
+        mb.step_tensors, mb.n_step_tensors = steps.data_ptr(), steps.numel()
+        mb.seed, mb.step_counter, mb.losses_ring = eng.seed, eng.step_counter.data_ptr(), eng.ring.data_ptr()
+        step0.append(float(steps.max().item()))
+        starts.append(eng.steps_done)
+        s.model.train()
+    ring_len = e0.ring.numel()
+    vals = np.empty((M, niters), dtype=np.float32)
+    stream = e0._stream()
+    size = C.sizeof(_native.PinnMember)
+
+    def drain(upto, drained):
+        torch.cuda.synchronize(e0.device)
+        for j, eng in enumerate(engines):
+            vals[j, drained:upto] = eng.ring.cpu().numpy()[(starts[j] + np.arange(drained, upto)) % ring_len]
+
+    done, drained = 0, 0
+    while done < niters:
+        kk = min(k, niters - done, ring_len)
+        if done + kk - drained > ring_len:
+            drain(done, drained)
+            drained = done
+        batches = []
+        if host_samplers is not None:
+            for j, smp in enumerate(host_samplers):
+                host = torch.empty((kk, batch_size, total), dtype=torch.float32).pin_memory()
+                for i in range(kk):
+                    b = smp.sample(batch_size)
+                    host[i].copy_(b if isinstance(b, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(b, dtype=np.float32)))
+                batches.append(host.to(e0.device, non_blocking=True))
+                members[j].points = batches[-1].data_ptr()
+        for j in range(M):
+            members[j].opt_step0 = step0[j] + done
+        for lo in range(0, M, _native.MAX_MEMBERS):
+            n = min(_native.MAX_MEMBERS, M - lo)
+            rc = lib.pinn_multi_step_ensemble(
+                e0.plan, n, C.cast(C.addressof(members) + lo * size, C.POINTER(_native.PinnMember)),
+                C.c_int64(batch_size), C.c_int(kk), C.c_float(lr), C.c_float(b1), C.c_float(b2), C.c_float(eps),
+                C.c_float(wd), C.c_int64(ring_len), C.c_float(point_weight), C.c_int(len(terms)), term_arr, cols, stream)
+            if rc == _native.E_UNSUPPORTED and done == 0 and lo == 0:
+                return lib.pinn_last_error().decode('utf-8', 'replace')
+            _native.check(rc)
+        done += kk
+    drain(niters, drained)
+    for j, (s, eng) in enumerate(zip(solvers, engines)):
+        eng.steps_done = starts[j] + niters
+        s.losses.extend(np.array(x, dtype=np.float32) for x in vals[j])
+    return None
