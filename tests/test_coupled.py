@@ -297,10 +297,13 @@ PICK = {
 ACTS = ['Tanh', 'Sigmoid', 'SiLU', 'GELU', 'Softplus']
 
 
-def random_coupled(seed, k=None, jet=None, kind=None):
+def random_coupled(seed, k=None, jet=None, kind=None, hidden=None, nparams=None, n=None):
     """ A random coupled problem: k outputs, one of the 15 jet sets (axis directions: the first ns carry a second
     derivative), V in the equation and / or the initial condition, dense or residual layout, one of five criteria.
-    `k`, `jet` = (nf, ns) and `kind` (criterion) may be fixed by the caller. """
+    `k`, `jet` = (nf, ns) and `kind` (criterion) may be fixed by the caller.  So may the hidden widths, the parameter
+    columns and the point count; they replace what was drawn after every draw, so a seed draws the same problem
+    otherwise.  `hidden`: an int (every hidden layer of the drawn layout) or a list of widths (a dense layout of that
+    many layers, the drawn activations in turn). """
     rng = np.random.RandomState(410000 + seed)
     nf, ns = jet if jet is not None else JET_SETS[seed % len(JET_SETS)]
     # k C reserved slots and k C partials: many channels leave room for fewer components in one 192-instruction program
@@ -308,18 +311,18 @@ def random_coupled(seed, k=None, jet=None, kind=None):
     k = k if k is not None else k_draw
     has_ic = bool(rng.rand() < 0.5)
     ndims = max(nf, 1) + (1 if has_ic and nf == 0 else 0)
-    nparams = int(rng.randint(2)) if ndims < 4 else 0
-    total = ndims + nparams
+    nparams_draw = int(rng.randint(2)) if ndims < 4 else 0
+    total = ndims + nparams_draw
     bc = None if rng.rand() < 0.4 else float(np.round(rng.uniform(-0.5, 0.5), 2))
     eq_var, ic_var = bool(rng.rand() < 0.5), bool(has_ic and rng.rand() < 0.5)
     coef = np.round(rng.uniform(0.2, 1.0, size=(k, 6)), 3)
     pick = list(PICK)[int(rng.randint(len(PICK)))]
-    hidden = int(rng.randint(4, 13))
+    width = int(rng.randint(4, 13))
     resnet = bool(rng.rand() < 0.4)
     n_act = 3 if resnet else 2
     acts = [ACTS[int(i)] for i in rng.randint(len(ACTS), size=n_act)]
     layout = 'faR fa fa+ f' if resnet else 'fafaf'
-    features = [hidden] * n_act + [k]
+    features = [width] * n_act + [k]
     kind_draw = ['mse', 'l1', 'huber', 'smooth_l1', 'mse_sum'][int(rng.randint(5))]
     kind = kind if kind is not None else kind_draw
 
@@ -353,11 +356,23 @@ def random_coupled(seed, k=None, jet=None, kind=None):
         variables['c'] = 0.6
     if ic_var and nsp > 0:
         variables['a'] = 0.7
-    n = int(rng.choice([1, 5, 33, 70]))
-    tag = 'k=%d nf=%d ns=%d ic=%s bc=%s %s %s %s %s n=%d' % (k, nf, ns, has_ic, bc, pick, layout, acts, kind, n)
+    n_draw = int(rng.choice([1, 5, 33, 70]))
+    log_scale = float(np.round(rng.uniform(-0.3, 0.3), 2))
+    # the caller's overrides, after the last draw
+    n = n_draw if n is None else n
+    if isinstance(hidden, int):
+        features = [hidden] * n_act + [k]
+    elif hidden is not None:
+        acts = [acts[i % n_act] for i in range(len(hidden))]
+        layout = 'fa' * len(hidden) + 'f'
+        features = list(hidden) + [k]
+    if nparams is not None:
+        total = ndims + nparams
+    nparams = nparams if nparams is not None else nparams_draw
+    tag ='k=%d nf=%d ns=%d ic=%s bc=%s %s %s %s %s n=%d' % (k, nf, ns, has_ic, bc, pick, layout, acts, kind, n)
     return dict(eq=eq, k=k, ndims=ndims, nparams=nparams, total=total, bc=bc, ic=ic, domain=domain, features=features,
                 acts=acts, layout=layout, variables=dict(sorted(variables.items())), kind=kind, n=n, tag=tag,
-                log_scale=float(np.round(rng.uniform(-0.3, 0.3), 2)), nf=nf, ns=ns)
+                log_scale=log_scale, nf=nf, ns=ns)
 
 
 def random_setup(seed, dtype=torch.float64, **fixed):
