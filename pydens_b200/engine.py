@@ -103,6 +103,42 @@ def shard_batch(batch_size, world, rank):
     return base + (1 if rank < rem else 0), rank * base + min(rank, rem)
 
 
+def sampler_columns(sampler, total):
+    """ Where a sampler's batches come from: (key, cols) with `cols` its in-kernel columns (None: the kernels' uniform
+    default) and `key` equal for samplers that draw the same columns, or (None, None): sampled on the host. """
+    if sampler is None:
+        return 'uniform', None
+    dev_cols = sampler.device_columns() if hasattr(sampler, 'device_columns') else None
+    if dev_cols is not None and len(dev_cols) == total and os.environ.get('PYDENS_B200_HOST_SAMPLER') != '1':
+        try:
+            cols = _native.make_columns(dev_cols, total)
+            return bytes(cols), cols
+        except ValueError:                    # more mixture components than the kernel takes
+            pass
+    return None, None
+
+
+def plain_adam(opt):
+    """ The optimizer is the Adam the kernels implement: torch.optim.Adam, one parameter group, no amsgrad, no
+    maximize, a float lr. """
+    g = opt.param_groups[0] if opt.param_groups else {}
+    return (type(opt) is torch.optim.Adam and len(opt.param_groups) == 1 and not g.get('amsgrad')
+            and not g.get('maximize') and not torch.is_tensor(g.get('lr')))
+
+
+def adam_hyper(opt):
+    """ (lr, (beta1, beta2), eps, weight_decay) of a plain_adam optimizer """
+    g = opt.param_groups[0]
+    return float(g['lr']), tuple(map(float, g['betas'])), float(g['eps']), float(g['weight_decay'])
+
+
+def auto_persistent(niters, batch_size, info):
+    """ A fit goes to the persistent kernels without steps_per_launch: tiny batches (launch- and latency-bound one step
+    at a time) and enough steps.  PYDENS_B200_AUTO_PERSISTENT=0 keeps one launch per step. """
+    return (niters >= _AUTO_PERSISTENT_MIN_ITERS and 0 < batch_size <= int(info.small_batch_points)
+            and os.environ.get('PYDENS_B200_AUTO_PERSISTENT', '1') != '0' and os.environ.get('PYDENS_B200_NO_GRAPH') != '1')
+
+
 class FusedEngine:
     def __init__(self, solver):
         self.lib = _native.load()
@@ -435,27 +471,17 @@ class FusedEngine:
             term_arr[i].points = e['host_points'].data_ptr()
         point_weight = 1.0 if total_sum else 1.0 / batch_size
         total = solver.model.total
-        g = opt.param_groups[0]
         mask = self._bind_adam_state(opt)
         m, v, steps, _ = self._adam_flat
         opt_step0 = float(steps.max().item())
-        cols, host_sampler = None, None
-        if sampler is not None:
-            dev_cols = sampler.device_columns() if hasattr(sampler, 'device_columns') else None
-            if dev_cols is not None and len(dev_cols) == total and os.environ.get('PYDENS_B200_HOST_SAMPLER') != '1':
-                try:
-                    cols = _native.make_columns(dev_cols, total)
-                except ValueError:
-                    cols = None
-            if cols is None:
-                host_sampler = sampler
+        cols_key, cols = sampler_columns(sampler, total)
+        host_sampler = sampler if cols_key is None else None
         solver.model.train()
         ring, ring_len = self.ring, self.ring.numel()
         start = self.steps_done
         vals = np.empty(niters, dtype=np.float32)
         done, drained = 0, 0
-        lr = float(g['lr']) if not torch.is_tensor(g['lr']) else float(g['lr'].item())
-        b1, b2 = g['betas']
+        lr, (b1, b2), eps, wd = adam_hyper(opt)
         while done < niters:
             kk = min(k, niters - done, ring_len)
             if done + kk - drained > ring_len:
@@ -475,7 +501,7 @@ class FusedEngine:
                 C.c_void_p(mask.data_ptr()), C.c_void_p(steps.data_ptr()), C.c_int(steps.numel()),
                 C.c_void_p(pts.data_ptr()) if pts is not None else None, cols, C.c_uint64(self.seed),
                 C.c_void_p(self.step_counter.data_ptr()), C.c_int64(batch_size), C.c_int(kk),
-                C.c_float(lr), C.c_float(b1), C.c_float(b2), C.c_float(g['eps']), C.c_float(g['weight_decay']),
+                C.c_float(lr), C.c_float(b1), C.c_float(b2), C.c_float(eps), C.c_float(wd),
                 C.c_float(opt_step0 + done), C.c_void_p(ring.data_ptr()), C.c_int64(ring_len),
                 C.c_float(point_weight), C.c_int(len(terms)), term_arr, self._stream())
             if rc == _native.E_UNSUPPORTED and done == 0 and terms:
@@ -498,26 +524,20 @@ class FusedEngine:
         # _AUTO_PERSISTENT_STEPS optimizer steps per launch (same math, same loss log; PYDENS_B200_AUTO_PERSISTENT=0
         # keeps one launch per step).  An explicit steps_per_launch takes precedence.
         requested = steps_per_launch > 0
-        if (not requested and niters >= _AUTO_PERSISTENT_MIN_ITERS and 0 < batch_size <= int(self.info.small_batch_points)
-                and os.environ.get('PYDENS_B200_AUTO_PERSISTENT', '1') != '0' and os.environ.get('PYDENS_B200_NO_GRAPH') != '1'):
+        if not requested and auto_persistent(niters, batch_size, self.info):
             steps_per_launch = _AUTO_PERSISTENT_STEPS
         if steps_per_launch > 0 and niters > 0:
-            g = opt.param_groups[0] if opt.param_groups else {}
             terms = None
-            if (type(opt) is torch.optim.Adam and len(opt.param_groups) == 1 and not g.get('amsgrad') and not g.get('maximize')
-                    and not torch.is_tensor(g.get('lr')) and _dist() is None and batch_size > 0):
+            if plain_adam(opt) and _dist() is None and batch_size > 0:
                 terms = self._persistent_terms(loss_terms, batch_size)
-            ok = terms is not None
-            if not ok and not requested:
-                steps_per_launch = 0
-            elif ok:
+            if terms is not None:
                 if solver.optimizer is not self._opt_obj:
                     self._drop_graphs()
                     self._opt_obj, self._opt_key = solver.optimizer, None
                 if self._fit_persistent(niters, batch_size, sampler, opt, steps_per_launch, terms):
                     return
-                if not requested:
-                    steps_per_launch = 0
+            if not requested:
+                steps_per_launch = 0
         if steps_per_launch > 0 and niters > 0:
             import warnings
             warnings.warn('pydens_b200: steps_per_launch ignored (needs Adam, one device, the equation term, constraints '
@@ -559,9 +579,7 @@ class FusedEngine:
         # optimizer.step() inside the step kernel (pinn_step_adam) whenever the optimizer is the plain torch Adam this
         # engine builds and nothing has to touch the gradient between the kernel and the update
         g0 = opt.param_groups[0] if opt.param_groups else {}
-        fused_adam = (os.environ.get('PYDENS_B200_FUSED_ADAM', '1') != '0' and type(opt) is torch.optim.Adam
-                      and len(opt.param_groups) == 1 and bool(g0.get('capturable')) and not g0.get('amsgrad')
-                      and not g0.get('maximize') and not torch.is_tensor(g0.get('lr'))
+        fused_adam = (os.environ.get('PYDENS_B200_FUSED_ADAM', '1') != '0' and plain_adam(opt) and bool(g0.get('capturable'))
                       and not fused_constraints and not nums and not stray_params and eq_term
                       and (dist is None or self.comm is not None))
         adam, adam_key = None, None
@@ -579,17 +597,8 @@ class FusedEngine:
             # all-reduce waits only a bounded time for its peers, so line the ranks up first
             dist.barrier()
 
-        cols, host_sampler, cols_key = None, None, None
-        if sampler is not None:
-            dev_cols = sampler.device_columns() if hasattr(sampler, 'device_columns') else None
-            if dev_cols is not None and len(dev_cols) == total and os.environ.get('PYDENS_B200_HOST_SAMPLER') != '1':
-                try:
-                    cols = _native.make_columns(dev_cols, total)
-                    cols_key = bytes(cols)
-                except ValueError:                    # more mixture components than the kernel takes
-                    cols = None
-            if cols is None:
-                host_sampler = sampler
+        cols_key, cols = sampler_columns(sampler, total)
+        host_sampler = sampler if cols_key is None else None
         solver.model.train()
 
         ring, ring_len = self.ring, self.ring.numel()

@@ -8,7 +8,6 @@ member keeps its own seed, optimizer state, frozen mask, loss list and step coun
 its solo fit.
 """
 import ctypes as C
-import os
 import warnings
 
 import numpy as np
@@ -16,7 +15,7 @@ import torch
 from torch import nn
 
 from . import _native
-from .engine import _AUTO_PERSISTENT_MIN_ITERS, _AUTO_PERSISTENT_STEPS, _dist
+from .engine import _AUTO_PERSISTENT_STEPS, _dist, adam_hyper, auto_persistent, plain_adam, sampler_columns
 
 # what each part of the problem's spec describes, for the error that names the difference between two members
 _SPEC_PARTS = (
@@ -61,20 +60,6 @@ def member_samplers(sampler, n):
             raise ValueError('fit_ensemble: %d samplers for %d solvers' % (len(sampler), n))
         return list(sampler)
     return [sampler] * n
-
-
-def _device_columns(sampler, total):
-    """ The in-kernel columns of a sampler as `_fit_persistent` takes them, or None: sampled on the host. """
-    if sampler is None:
-        return 'uniform', None
-    dev_cols = sampler.device_columns() if hasattr(sampler, 'device_columns') else None
-    if dev_cols is not None and len(dev_cols) == total and os.environ.get('PYDENS_B200_HOST_SAMPLER') != '1':
-        try:
-            cols = _native.make_columns(dev_cols, total)
-            return bytes(cols), cols
-        except ValueError:
-            pass
-    return None, None
 
 
 def fit_ensemble(solvers, niters, batch_size, sampler=None, loss_terms='equation', optimizer='Adam',
@@ -130,8 +115,7 @@ def _fit_together(solvers, niters, batch_size, samplers, loss_terms, optimizer, 
     e0 = engines[0]
     k = int(steps_per_launch or 0)
     if k <= 0:                                            # the rule of FusedEngine.fit for tiny batches
-        if not (niters >= _AUTO_PERSISTENT_MIN_ITERS and 0 < batch_size <= int(e0.info.small_batch_points)
-                and os.environ.get('PYDENS_B200_AUTO_PERSISTENT', '1') != '0' and os.environ.get('PYDENS_B200_NO_GRAPH') != '1'):
+        if not auto_persistent(niters, batch_size, e0.info):
             return ('a solo fit of batch %d x %d steps does not take the persistent kernels by itself '
                     '(pass steps_per_launch)' % (batch_size, niters))
         k = _AUTO_PERSISTENT_STEPS
@@ -149,7 +133,7 @@ def _fit_together(solvers, niters, batch_size, samplers, loss_terms, optimizer, 
             if diff is not None:
                 raise ValueError('fit_ensemble: solver %d differs from solver 0 in constraint %d: %s' % (j, i, diff))
     total = solvers[0].model.total
-    keys = [_device_columns(smp, total) for smp in samplers]
+    keys = [sampler_columns(smp, total) for smp in samplers]
     if len({key for key, _ in keys}) > 1:
         return 'the members\' samplers differ in their in-kernel columns, or some sample on the host'
     cols = keys[0][1]
@@ -157,13 +141,10 @@ def _fit_together(solvers, niters, batch_size, samplers, loss_terms, optimizer, 
     opts = []
     for eng in engines:
         opt, _ = eng._optimizer_for(optimizer, lr, dict(kwargs))
-        g = opt.param_groups[0] if opt.param_groups else {}
-        if not (type(opt) is torch.optim.Adam and len(opt.param_groups) == 1 and not g.get('amsgrad')
-                and not g.get('maximize') and not torch.is_tensor(g.get('lr'))):
+        if not plain_adam(opt):
             return 'the optimizer is not plain torch.optim.Adam with one parameter group'
         opts.append(opt)
-    hyper = [(float(o.param_groups[0]['lr']), tuple(map(float, o.param_groups[0]['betas'])),
-              float(o.param_groups[0]['eps']), float(o.param_groups[0]['weight_decay'])) for o in opts]
+    hyper = [adam_hyper(o) for o in opts]
     if len(set(hyper)) > 1:
         return 'the members\' Adam hyper-parameters differ'
     return _run(solvers, engines, opts, terms[0], niters, batch_size, samplers if host else None, cols, k, hyper[0])
