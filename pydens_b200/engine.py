@@ -13,11 +13,13 @@ The sequence is captured once in a CUDA graph and replayed; nothing in it touche
 """
 import ctypes as C
 import os
+import warnings
 
 import numpy as np
 import torch
 
 from . import _native
+from .solver import _progress
 
 _GRAPH_MIN_ITERS = 8
 _HOST_GRAPH_MIN_ITERS = 8           # host-sampler mode: one capture per staging buffer
@@ -137,6 +139,96 @@ def auto_persistent(niters, batch_size, info):
     at a time) and enough steps.  PYDENS_B200_AUTO_PERSISTENT=0 keeps one launch per step. """
     return (niters >= _AUTO_PERSISTENT_MIN_ITERS and 0 < batch_size <= int(info.small_batch_points)
             and os.environ.get('PYDENS_B200_AUTO_PERSISTENT', '1') != '0' and os.environ.get('PYDENS_B200_NO_GRAPH') != '1')
+
+
+def ring_losses(ring, start, lo, hi):
+    """ The losses of steps [lo, hi) of a fit whose first step went to ring entry `start` (modulo the ring's length),
+    read from the device loss ring; the caller has synchronised the device. """
+    return ring.cpu().numpy()[(start + np.arange(lo, hi)) % ring.numel()]
+
+
+def run_persistent(engines, opts, samplers, terms, niters, batch_size, k, table):
+    """ `niters` optimizer steps of every engine's fit, `k` per launch of the persistent multi-step kernels: the
+    reference loop model_torch.py:426-464 with optimizer.step() inside the kernel, constraint terms included.  One fit
+    runs on the solo kernels (pinn_multi_step_terms) unless `table` is set; with `table` the fits are members of
+    pinn_multi_step_ensemble, at most MAX_MEMBERS per launch.  `samplers` has one sampler per fit: all in-kernel with
+    the same columns, or all on the host.  Returns None, or the library's message when it refused the first launch
+    with PINN_E_UNSUPPORTED (no step has been taken then). """
+    e0 = engines[0]
+    lib, total, ring_len = e0.lib, e0.solver.model.total, e0.ring.numel()
+    # point weights: the mean of model_torch.py:448 over the batch and over every constraint's own points, or 1
+    total_sum = e0._sum_reduction()
+    term_arr = (_native.PinnTerm * max(1, len(terms)))()
+    for i, e in enumerate(terms):
+        term_arr[i].plan = e['plan'].value
+        term_arr[i].n_points = e['n']
+        term_arr[i].point_weight = 1.0 if total_sum else 1.0 / e['n']
+        term_arr[i].points = e['host_points'].data_ptr()
+    point_weight = 1.0 if total_sum else 1.0 / batch_size
+    M = len(engines)
+    members = (_native.PinnMember * M)()
+    starts, step0 = [], []
+    for mb, eng, opt in zip(members, engines, opts):
+        eng._adopt_optimizer()
+        mask = eng._bind_adam_state(opt)
+        m, v, steps, _ = eng._adam_flat
+        mb.params, mb.exp_avg, mb.exp_avg_sq, mb.mask = eng.flat.data_ptr(), m.data_ptr(), v.data_ptr(), mask.data_ptr()
+        mb.step_tensors, mb.n_step_tensors = steps.data_ptr(), steps.numel()
+        mb.seed, mb.step_counter, mb.losses_ring = eng.seed, eng.step_counter.data_ptr(), eng.ring.data_ptr()
+        step0.append(float(steps.max().item()))
+        starts.append(eng.steps_done)
+        eng.solver.model.train()
+    cols_key, cols = sampler_columns(samplers[0], total)
+    host = cols_key is None
+    lr, (b1, b2), eps, wd = adam_hyper(opts[0])
+    stream = e0._stream()
+    size = C.sizeof(_native.PinnMember)
+    vals = np.empty((M, niters), dtype=np.float32)
+
+    def drain(lo, hi):
+        torch.cuda.synchronize(e0.device)
+        for j, eng in enumerate(engines):
+            vals[j, lo:hi] = ring_losses(eng.ring, starts[j], lo, hi)
+
+    done, drained = 0, 0
+    while done < niters:
+        kk = min(k, niters - done, ring_len)
+        if done + kk - drained > ring_len:
+            drain(drained, done)
+            drained = done
+        batches = []                                      # each member's kk batches, alive until the launch
+        for mb, smp, s0 in zip(members, samplers, step0):
+            if host:
+                pinned = torch.empty((kk, batch_size, total), dtype=torch.float32).pin_memory()
+                for i in range(kk):
+                    b = smp.sample(batch_size)
+                    pinned[i].copy_(b if isinstance(b, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(b, dtype=np.float32)))
+                batches.append(pinned.to(e0.device, non_blocking=True))
+                mb.points = batches[-1].data_ptr()
+            mb.opt_step0 = s0 + done
+        for lo in range(0, M, _native.MAX_MEMBERS):
+            if table:
+                rc = lib.pinn_multi_step_ensemble(
+                    e0.plan, min(_native.MAX_MEMBERS, M - lo),
+                    C.cast(C.addressof(members) + lo * size, C.POINTER(_native.PinnMember)), C.c_int64(batch_size),
+                    C.c_int(kk), C.c_float(lr), C.c_float(b1), C.c_float(b2), C.c_float(eps), C.c_float(wd),
+                    C.c_int64(ring_len), C.c_float(point_weight), C.c_int(len(terms)), term_arr, cols, stream)
+            else:
+                mb = members[0]
+                rc = lib.pinn_multi_step_terms(
+                    e0.plan, mb.params, mb.exp_avg, mb.exp_avg_sq, mb.mask, mb.step_tensors, mb.n_step_tensors,
+                    mb.points, cols, mb.seed, mb.step_counter, C.c_int64(batch_size), C.c_int(kk), C.c_float(lr),
+                    C.c_float(b1), C.c_float(b2), C.c_float(eps), C.c_float(wd), C.c_float(mb.opt_step0),
+                    mb.losses_ring, C.c_int64(ring_len), C.c_float(point_weight), C.c_int(len(terms)), term_arr, stream)
+            if rc == _native.E_UNSUPPORTED and done == 0 and lo == 0:
+                return lib.pinn_last_error().decode('utf-8', 'replace')
+            _native.check(rc)
+        done += kk
+    drain(drained, niters)
+    for j, eng in enumerate(engines):
+        eng.steps_done = starts[j] + niters
+        eng.solver.losses.extend(np.array(x, dtype=np.float32) for x in vals[j])
+    return None
 
 
 class FusedEngine:
@@ -391,6 +483,13 @@ class FusedEngine:
         self._opt_obj, self._opt_key = solver.optimizer, key
         return solver.optimizer, False
 
+    def _adopt_optimizer(self):
+        """ The solver's optimizer was not built by _optimizer_for (optimizer=None with an optimizer built elsewhere):
+        the captured graphs hold pointers into another optimizer's state, and no request matches this one. """
+        if self.solver.optimizer is not self._opt_obj:
+            self._drop_graphs()
+            self._opt_obj, self._opt_key = self.solver.optimizer, None
+
     def _drop_graphs(self):
         self._graphs = {}
         for pipe in getattr(self, '_pipes', {}).values():
@@ -457,66 +556,16 @@ class FusedEngine:
         return entries
 
     def _fit_persistent(self, niters, batch_size, sampler, opt, k, terms=()):
-        """ `niters` optimizer steps, `k` per launch of the persistent multi-step kernel (pinn_multi_step_terms):
-        the reference loop model_torch.py:426-464 with optimizer.step() inside the kernel, constraint terms included.
+        """ `niters` optimizer steps, `k` per launch of the solo persistent multi-step kernels (run_persistent).
         Returns False, having taken no step, when the kernels cannot hold the constraint programs' scratch slots. """
-        solver = self.solver
-        # point weights: the mean of model_torch.py:448 over the batch and over every constraint's own points, or 1
-        total_sum = self._sum_reduction()
-        term_arr = (_native.PinnTerm * max(1, len(terms)))()
-        for i, e in enumerate(terms):
-            term_arr[i].plan = e['plan'].value
-            term_arr[i].n_points = e['n']
-            term_arr[i].point_weight = 1.0 if total_sum else 1.0 / e['n']
-            term_arr[i].points = e['host_points'].data_ptr()
-        point_weight = 1.0 if total_sum else 1.0 / batch_size
-        total = solver.model.total
-        mask = self._bind_adam_state(opt)
-        m, v, steps, _ = self._adam_flat
-        opt_step0 = float(steps.max().item())
-        cols_key, cols = sampler_columns(sampler, total)
-        host_sampler = sampler if cols_key is None else None
-        solver.model.train()
-        ring, ring_len = self.ring, self.ring.numel()
-        start = self.steps_done
-        vals = np.empty(niters, dtype=np.float32)
-        done, drained = 0, 0
-        lr, (b1, b2), eps, wd = adam_hyper(opt)
-        while done < niters:
-            kk = min(k, niters - done, ring_len)
-            if done + kk - drained > ring_len:
-                torch.cuda.synchronize(self.device)
-                idx = (start + np.arange(drained, done)) % ring_len
-                vals[drained:done] = ring.cpu().numpy()[idx]
-                drained = done
-            pts = None
-            if host_sampler is not None:
-                host = torch.empty((kk, batch_size, total), dtype=torch.float32).pin_memory()
-                for j in range(kk):
-                    b = host_sampler.sample(batch_size)
-                    host[j].copy_(b if isinstance(b, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(b, dtype=np.float32)))
-                pts = host.to(self.device, non_blocking=True)
-            rc = self.lib.pinn_multi_step_terms(
-                self.plan, C.c_void_p(self.flat.data_ptr()), C.c_void_p(m.data_ptr()), C.c_void_p(v.data_ptr()),
-                C.c_void_p(mask.data_ptr()), C.c_void_p(steps.data_ptr()), C.c_int(steps.numel()),
-                C.c_void_p(pts.data_ptr()) if pts is not None else None, cols, C.c_uint64(self.seed),
-                C.c_void_p(self.step_counter.data_ptr()), C.c_int64(batch_size), C.c_int(kk),
-                C.c_float(lr), C.c_float(b1), C.c_float(b2), C.c_float(eps), C.c_float(wd),
-                C.c_float(opt_step0 + done), C.c_void_p(ring.data_ptr()), C.c_int64(ring_len),
-                C.c_float(point_weight), C.c_int(len(terms)), term_arr, self._stream())
-            if rc == _native.E_UNSUPPORTED and done == 0 and terms:
-                return False
-            _native.check(rc)
-            done += kk
-        self.steps_done = start + niters
-        torch.cuda.synchronize(self.device)
-        idx = (start + np.arange(drained, niters)) % ring_len
-        vals[drained:niters] = ring.cpu().numpy()[idx]
-        solver.losses.extend(np.array(x, dtype=np.float32) for x in vals)
-        return True
+        refused = run_persistent([self], [opt], [sampler], terms, niters, batch_size, k, table=False)
+        if refused is None:
+            return True
+        if terms:
+            return False
+        raise _native.NativeError(_native.E_UNSUPPORTED, refused)
 
     def fit(self, niters, batch_size, sampler, loss_terms, optimizer, criterion, lr, **kwargs):
-        solver = self.solver
         steps_per_launch = int(kwargs.pop('steps_per_launch', 0) or 0)
         opt, opt_ready = self._optimizer_for(optimizer, lr, kwargs)
         # Tiny batches (the README example: batch_size=100, niters=1500) are launch- and latency-bound one step at a
@@ -530,24 +579,21 @@ class FusedEngine:
             terms = None
             if plain_adam(opt) and _dist() is None and batch_size > 0:
                 terms = self._persistent_terms(loss_terms, batch_size)
-            if terms is not None:
-                if solver.optimizer is not self._opt_obj:
-                    self._drop_graphs()
-                    self._opt_obj, self._opt_key = solver.optimizer, None
-                if self._fit_persistent(niters, batch_size, sampler, opt, steps_per_launch, terms):
-                    return
-            if not requested:
-                steps_per_launch = 0
-        if steps_per_launch > 0 and niters > 0:
-            import warnings
-            warnings.warn('pydens_b200: steps_per_launch ignored (needs Adam, one device, the equation term, constraints '
-                          'that run fused (at most %d, with %d points in all), batch + constraint points of at most %d '
-                          'and a network that fits the persistent kernel)'
-                          % (_native.MAX_TERMS, _native.MAX_TERM_POINTS, self.lib.pinn_multi_step_max_points(self.plan)),
-                          stacklevel=3)
-        if solver.optimizer is not self._opt_obj:          # optimizer=None with an optimizer built elsewhere
-            self._drop_graphs()
-            self._opt_obj, self._opt_key = solver.optimizer, None
+            if terms is not None and self._fit_persistent(niters, batch_size, sampler, opt, steps_per_launch, terms):
+                return
+            if requested:
+                warnings.warn('pydens_b200: steps_per_launch ignored (needs Adam, one device, the equation term, '
+                              'constraints that run fused (at most %d, with %d points in all), batch + constraint points '
+                              'of at most %d and a network that fits the persistent kernel)'
+                              % (_native.MAX_TERMS, _native.MAX_TERM_POINTS,
+                                 self.lib.pinn_multi_step_max_points(self.plan)), stacklevel=3)
+        self._fit_stepwise(niters, batch_size, sampler, loss_terms, criterion, opt, opt_ready)
+
+    def _fit_stepwise(self, niters, batch_size, sampler, loss_terms, criterion, opt, opt_ready):
+        """ One launch of the step kernel per optimizer step, with the constraint launches, autograd's constraints and
+        torch's optimizer (or the Adam in the step kernel's tail); captured in CUDA graphs where possible. """
+        solver = self.solver
+        self._adopt_optimizer()
         nums = solver._constraint_numbers(loss_terms)
         eq_term = 'equation' in loss_terms                # reference :448: the equation term is optional (:382-389)
         fused_constraints = [e for e in (self._constraint_plan(n) for n in nums) if e is not None]
@@ -578,18 +624,18 @@ class FusedEngine:
 
         # optimizer.step() inside the step kernel (pinn_step_adam) whenever the optimizer is the plain torch Adam this
         # engine builds and nothing has to touch the gradient between the kernel and the update
-        g0 = opt.param_groups[0] if opt.param_groups else {}
-        fused_adam = (os.environ.get('PYDENS_B200_FUSED_ADAM', '1') != '0' and plain_adam(opt) and bool(g0.get('capturable'))
+        capturable = bool(opt.param_groups and opt.param_groups[0].get('capturable', False))
+        fused_adam = (os.environ.get('PYDENS_B200_FUSED_ADAM', '1') != '0' and plain_adam(opt) and capturable
                       and not fused_constraints and not nums and not stray_params and eq_term
                       and (dist is None or self.comm is not None))
         adam, adam_key = None, None
         if fused_adam:
             mask = self._bind_adam_state(opt)          # the optimizer's state tensors become views of flat buffers
             m_flat, v_flat, steps_flat, _ = self._adam_flat
+            adam_key = adam_hyper(opt)
+            lr, (b1, b2), eps, wd = adam_key
             adam = _native.PinnAdam(m_flat.data_ptr(), v_flat.data_ptr(), mask.data_ptr(), steps_flat.data_ptr(),
-                                    steps_flat.numel(), float(g0['lr']), float(g0['betas'][0]), float(g0['betas'][1]),
-                                    float(g0['eps']), float(g0['weight_decay']), self.ring.data_ptr(), self.ring.numel())
-            adam_key = (float(g0['lr']), tuple(float(b) for b in g0['betas']), float(g0['eps']), float(g0['weight_decay']))
+                                    steps_flat.numel(), lr, b1, b2, eps, wd, self.ring.data_ptr(), self.ring.numel())
             opt_ready = True                           # the state exists (zeros for a fresh optimizer)
 
         if dist is not None:
@@ -598,23 +644,9 @@ class FusedEngine:
             dist.barrier()
 
         cols_key, cols = sampler_columns(sampler, total)
-        host_sampler = sampler if cols_key is None else None
         solver.model.train()
-
-        ring, ring_len = self.ring, self.ring.numel()
-        start = self.steps_done
         loss_idx = self.n_params
-        stream = self._stream()
-        ring_ptr = ring.data_ptr()
-        vals = np.empty(niters, dtype=np.float32)
-        drained = [0]
-
-        def drain(upto):
-            """ losses of steps [drained, upto) of this fit: device ring -> vals (the ring has been synchronised) """
-            if upto > drained[0]:
-                idx = (start + np.arange(drained[0], upto)) % ring_len
-                vals[drained[0]:upto] = ring.cpu().numpy()[idx]
-                drained[0] = upto
+        ring_ptr, ring_len = self.ring.data_ptr(), self.ring.numel()
 
         def one_step(points=None, full_points=None):
             if fused_adam:
@@ -647,129 +679,142 @@ class FusedEngine:
                                                     C.c_void_p(ring_ptr), C.c_int64(ring_len),
                                                     C.c_void_p(self.step_counter.data_ptr()), self._stream()))
 
-        capturable = bool(opt.param_groups and opt.param_groups[0].get('capturable', False))
         graphs_ok = (capturable or fused_adam) and not nums and os.environ.get('PYDENS_B200_NO_GRAPH') != '1'
-        from .solver import _progress
-        done = 0
+        if cols_key is not None:
+            vals = self._loop_in_kernel_sampler(niters, one_step, graphs_ok, opt_ready,
+                                                ('dev', batch_size, local_n, cols_key, fused_nums, adam_key))
+        else:
+            vals = self._loop_host_batches(niters, batch_size, local_n, point_offset, sampler, one_step, graphs_ok,
+                                           ('host', batch_size, local_n, fused_nums, adam_key), nums, dist)
+        self._end_stepwise(vals, dist)
 
-        if host_sampler is None:
-            # ---------------- points sampled in the kernel: replay graphs of `per_graph` steps ----------------
-            per_graph = int(os.environ.get('PYDENS_B200_GRAPH_STEPS', '0')) or (4 if niters >= 64 else 1)
-            key = ('dev', batch_size, local_n, cols_key, fused_nums, per_graph, adam_key)
-            graph = self._graphs.get(key) if graphs_ok else None
-            if graphs_ok and graph is None and niters >= _GRAPH_MIN_ITERS:
-                if not opt_ready:
-                    one_step()                        # real step 0: also materialises optimizer state
-                    done = 1
+    def _loop_in_kernel_sampler(self, niters, one_step, graphs_ok, opt_ready, key):
+        """ Points sampled in the kernel: replays of a graph of `per_graph` steps, the rest as plain launches.
+        -> the losses of the `niters` steps """
+        ring_len, start = self.ring.numel(), self.steps_done
+        vals = np.empty(niters, dtype=np.float32)
+        per_graph = int(os.environ.get('PYDENS_B200_GRAPH_STEPS', '0')) or (4 if niters >= 64 else 1)
+        key += (per_graph,)
+        graph = self._graphs.get(key) if graphs_ok else None
+        done, drained = 0, 0
+        if graphs_ok and graph is None and niters >= _GRAPH_MIN_ITERS:
+            if not opt_ready:
+                one_step()                        # real step 0: also materialises optimizer state
+                done = 1
+            try:
+                torch.cuda.synchronize(self.device)
+
+                def body():
+                    for _ in range(per_graph):
+                        one_step()
+                # capture executes nothing, but a first launch of a freshly captured kernel sequence must not
+                # be preceded by a dry run: the capture itself is side-effect free
+                graph = capture_graph(self.device, body)
+                self._graphs[key] = graph
+            except Exception as exc:              # capture unsupported here: plain launches  # noqa: BLE001
+                warnings.warn('pydens_b200: CUDA-graph capture of the step failed (%s); using plain launches' % exc)
+                graph = None
+                torch.cuda.synchronize(self.device)
+        if graph is not None:
+            for _ in range((niters - done) // per_graph):
+                if done + per_graph - drained > ring_len:     # the ring is about to wrap: read it out first
+                    torch.cuda.synchronize(self.device)
+                    vals[drained:done] = ring_losses(self.ring, start, drained, done)
+                    drained = done
+                graph.replay()
+                done += per_graph
+        for _ in _progress(niters - done):
+            if done - drained >= ring_len:
+                torch.cuda.synchronize(self.device)
+                vals[drained:done] = ring_losses(self.ring, start, drained, done)
+                drained = done
+            one_step()
+            done += 1
+        torch.cuda.synchronize(self.device)
+        vals[drained:] = ring_losses(self.ring, start, drained, niters)
+        return vals
+
+    def _loop_host_batches(self, niters, batch_size, local_n, point_offset, host_sampler, one_step, graphs_ok, key,
+                           nums, dist):
+        """ Host batches through the native pipeline, one call per step (copy -> graph -> loss read once the graphs
+        are captured).  -> the losses of the `niters` steps """
+        total, start, stream = self.solver.model.total, self.steps_done, self._stream()
+        ring_ptr, ring_len = self.ring.data_ptr(), self.ring.numel()
+        # staging depth = how many steps the host may run ahead of the GPU (absorbs host jitter; matters most
+        # with several ranks, where the in-kernel all-reduce makes every rank wait for the slowest host)
+        n_stage = max(2, min(8, int(os.environ.get('PYDENS_B200_STAGES', '4'))))
+        pkey = (local_n, n_stage)
+        pipe = self._pipes.get(pkey)
+        if pipe is None:
+            pipe = C.c_void_p()
+            _native.check(self.lib.pinn_pipe_create(self.plan, n_stage, C.c_int64(local_n), C.byref(pipe)))
+            self._pipes[pkey] = pipe
+        bufs = [_RawPtr(self.lib.pinn_pipe_buffer(pipe, k)) for k in range(n_stage)]
+        pinned = self._pinned_batches.get((batch_size, n_stage))
+        loss_host = self._pinned_losses(niters)
+        loss_ptr = loss_host.data_ptr()
+        key += (n_stage,)
+        execs = self._graphs.get(key) if graphs_ok else None
+        exec_ptrs = [g.raw_cuda_graph_exec() for g in execs] if execs else None
+        keep = [None] * n_stage                    # the tensors whose memory a copy in flight still reads
+        off_bytes = point_offset * total * 4
+        want_graphs = graphs_ok and execs is None and niters >= _HOST_GRAPH_MIN_ITERS
+
+        for i in _progress(niters):
+            k = i % n_stage
+            batch = host_sampler.sample(batch_size)
+            if isinstance(batch, torch.Tensor) and batch.dtype == torch.float32 and batch.is_contiguous() \
+                    and batch.device.type == 'cpu':
+                src = batch                        # copied from where it lies (pinned or not)
+            else:
+                if pinned is None:
+                    pinned = [torch.empty((batch_size, total), dtype=torch.float32).pin_memory()
+                              for _ in range(n_stage)]
+                    self._pinned_batches[(batch_size, n_stage)] = pinned
+                _native.check(self.lib.pinn_pipe_wait(pipe, k))          # its previous copy has left the buffer
+                if isinstance(batch, torch.Tensor):
+                    pinned[k].copy_(batch.detach().to('cpu', torch.float32).reshape(batch_size, total))
+                else:
+                    pinned[k].copy_(torch.from_numpy(np.ascontiguousarray(batch, dtype=np.float32)).reshape(batch_size, total))
+                src = pinned[k]
+            keep[k] = src
+            r = (start + i) % ring_len
+            if exec_ptrs is not None:
+                _native.check(self.lib.pinn_pipe_step(pipe, k, C.c_void_p(src.data_ptr() + off_bytes),
+                                                      C.c_void_p(exec_ptrs[k]), C.c_void_p(ring_ptr + 4 * r),
+                                                      C.c_void_p(loss_ptr + 4 * i), stream))
+                continue
+            _native.check(self.lib.pinn_pipe_step(pipe, k, C.c_void_p(src.data_ptr() + off_bytes), None, None, None, stream))
+            full = None
+            if nums:
+                full = src.to(self.device, non_blocking=True)
+                if dist is not None:
+                    dist.broadcast(full, 0)
+            one_step(bufs[k], full)
+            _native.check(self.lib.pinn_pipe_finish(pipe, k, C.c_void_p(ring_ptr + 4 * r), C.c_void_p(loss_ptr + 4 * i), stream))
+            # after the first (eager) step the optimizer state exists: capture the compute part of the step
+            # once per staging buffer, so that every later step is ONE native call (copy -> graph -> loss read)
+            if want_graphs:
+                want_graphs = False
                 try:
                     torch.cuda.synchronize(self.device)
-
-                    def body():
-                        for _ in range(per_graph):
-                            one_step()
-                    # capture executes nothing, but a first launch of a freshly captured kernel sequence must not
-                    # be preceded by a dry run: the capture itself is side-effect free
-                    graph = capture_graph(self.device, body)
-                    self._graphs[key] = graph
-                except Exception as exc:              # capture unsupported here: plain launches  # noqa: BLE001
-                    import warnings
+                    graphs = []
+                    for kk in range(n_stage):
+                        graphs.append(capture_graph(self.device, lambda kk=kk: one_step(bufs[kk]),
+                                                    pool=graphs[0].pool() if graphs else None))
+                    self._graphs[key] = graphs
+                    exec_ptrs = [g.raw_cuda_graph_exec() for g in graphs]
+                except Exception as exc:        # capture unsupported here: keep plain launches  # noqa: BLE001
                     warnings.warn('pydens_b200: CUDA-graph capture of the step failed (%s); using plain launches' % exc)
-                    graph = None
+                    exec_ptrs = None
                     torch.cuda.synchronize(self.device)
-            if graph is not None:
-                n_rep = (niters - done) // per_graph
-                budget = ring_len - done
-                for _ in range(n_rep):
-                    if budget < per_graph:            # the ring is about to wrap: read it out first
-                        torch.cuda.synchronize(self.device)
-                        drain(done)
-                        budget = ring_len
-                    graph.replay()
-                    done += per_graph
-                    budget -= per_graph
-            for _ in _progress(niters - done):
-                if done - drained[0] >= ring_len:
-                    torch.cuda.synchronize(self.device)
-                    drain(done)
-                one_step()
-                done += 1
-            self.steps_done = start + niters
-            torch.cuda.synchronize(self.device)
-            drain(niters)
-        else:
-            # ---------------- host batches: native pipeline, one call per step ----------------
-            # staging depth = how many steps the host may run ahead of the GPU (absorbs host jitter; matters most
-            # with several ranks, where the in-kernel all-reduce makes every rank wait for the slowest host)
-            n_stage = max(2, min(8, int(os.environ.get('PYDENS_B200_STAGES', '4'))))
-            pkey = (local_n, n_stage)
-            pipe = self._pipes.get(pkey)
-            if pipe is None:
-                pipe = C.c_void_p()
-                _native.check(self.lib.pinn_pipe_create(self.plan, n_stage, C.c_int64(local_n), C.byref(pipe)))
-                self._pipes[pkey] = pipe
-            bufs = [_RawPtr(self.lib.pinn_pipe_buffer(pipe, k)) for k in range(n_stage)]
-            pinned = self._pinned_batches.get((batch_size, n_stage))
-            loss_host = self._pinned_losses(niters)
-            loss_ptr = loss_host.data_ptr()
-            key = ('host', batch_size, local_n, n_stage, fused_nums, adam_key)
-            execs = self._graphs.get(key) if graphs_ok else None
-            exec_ptrs = [g.raw_cuda_graph_exec() for g in execs] if execs else None
-            keep = [None] * n_stage                    # the tensors whose memory a copy in flight still reads
-            off_bytes = point_offset * total * 4
-            want_graphs = graphs_ok and execs is None and niters >= _HOST_GRAPH_MIN_ITERS
+        torch.cuda.synchronize(self.device)
+        return loss_host[:niters].numpy().copy()
 
-            for i in _progress(niters):
-                k = i % n_stage
-                batch = host_sampler.sample(batch_size)
-                if isinstance(batch, torch.Tensor) and batch.dtype == torch.float32 and batch.is_contiguous() \
-                        and batch.device.type == 'cpu':
-                    src = batch                        # copied from where it lies (pinned or not)
-                else:
-                    if pinned is None:
-                        pinned = [torch.empty((batch_size, total), dtype=torch.float32).pin_memory()
-                                  for _ in range(n_stage)]
-                        self._pinned_batches[(batch_size, n_stage)] = pinned
-                    _native.check(self.lib.pinn_pipe_wait(pipe, k))          # its previous copy has left the buffer
-                    if isinstance(batch, torch.Tensor):
-                        pinned[k].copy_(batch.detach().to('cpu', torch.float32).reshape(batch_size, total))
-                    else:
-                        pinned[k].copy_(torch.from_numpy(np.ascontiguousarray(batch, dtype=np.float32)).reshape(batch_size, total))
-                    src = pinned[k]
-                keep[k] = src
-                r = (start + i) % ring_len
-                if exec_ptrs is not None:
-                    _native.check(self.lib.pinn_pipe_step(pipe, k, C.c_void_p(src.data_ptr() + off_bytes),
-                                                          C.c_void_p(exec_ptrs[k]), C.c_void_p(ring_ptr + 4 * r),
-                                                          C.c_void_p(loss_ptr + 4 * i), stream))
-                    continue
-                _native.check(self.lib.pinn_pipe_step(pipe, k, C.c_void_p(src.data_ptr() + off_bytes), None, None, None, stream))
-                full = None
-                if nums:
-                    full = src.to(self.device, non_blocking=True)
-                    if dist is not None:
-                        dist.broadcast(full, 0)
-                one_step(bufs[k], full)
-                _native.check(self.lib.pinn_pipe_finish(pipe, k, C.c_void_p(ring_ptr + 4 * r), C.c_void_p(loss_ptr + 4 * i), stream))
-                # after the first (eager) step the optimizer state exists: capture the compute part of the step
-                # once per staging buffer, so that every later step is ONE native call (copy -> graph -> loss read)
-                if want_graphs:
-                    want_graphs = False
-                    try:
-                        torch.cuda.synchronize(self.device)
-                        graphs = []
-                        for kk in range(n_stage):
-                            graphs.append(capture_graph(self.device, lambda kk=kk: one_step(bufs[kk]),
-                                                        pool=graphs[0].pool() if graphs else None))
-                        self._graphs[key] = graphs
-                        exec_ptrs = [g.raw_cuda_graph_exec() for g in graphs]
-                    except Exception as exc:        # capture unsupported here: keep plain launches  # noqa: BLE001
-                        import warnings
-                        warnings.warn('pydens_b200: CUDA-graph capture of the step failed (%s); using plain launches' % exc)
-                        exec_ptrs = None
-                        torch.cuda.synchronize(self.device)
-            self.steps_done = start + niters
-            torch.cuda.synchronize(self.device)
-            vals[:] = loss_host[:niters].numpy()
+    def _end_stepwise(self, vals, dist):
+        """ The end of a stepwise fit of len(vals) steps: drop graphs that hold NCCL collectives, check that every
+        rank reached the in-kernel all-reduce, log the losses. """
+        self.steps_done += len(vals)
         if dist is not None and self.comm is None:
             # NCCL fallback: the cached graphs hold captured NCCL collectives, and NCCL's communicator teardown
             # (dist.destroy_process_group) waits for every such graph to be destroyed first — do not keep them
@@ -780,7 +825,7 @@ class FusedEngine:
             if aborted.value:
                 raise RuntimeError('pydens_b200: a rank did not reach the in-kernel all-reduce within the time limit '
                                    '(PINN_COMM_TIMEOUT_S); the gradients of this fit were poisoned with NaN')
-        solver.losses.extend(np.array(v, dtype=np.float32) for v in vals[:niters])
+        self.solver.losses.extend(np.array(v, dtype=np.float32) for v in vals)
 
 
 class _RawPtr:

@@ -7,15 +7,13 @@ cluster of at most 8 CTAs; `fit_ensemble` puts up to PINN_MAX_MEMBERS of them in
 member keeps its own seed, optimizer state, frozen mask, loss list and step counter, and its result is bit-identical to
 its solo fit.
 """
-import ctypes as C
 import warnings
 
-import numpy as np
-import torch
 from torch import nn
 
 from . import _native
-from .engine import _AUTO_PERSISTENT_STEPS, _dist, adam_hyper, auto_persistent, plain_adam, sampler_columns
+from .engine import (_AUTO_PERSISTENT_STEPS, _dist, adam_hyper, auto_persistent, plain_adam, run_persistent,
+                     sampler_columns)
 
 # what each part of the problem's spec describes, for the error that names the difference between two members
 _SPEC_PARTS = (
@@ -133,92 +131,15 @@ def _fit_together(solvers, niters, batch_size, samplers, loss_terms, optimizer, 
             if diff is not None:
                 raise ValueError('fit_ensemble: solver %d differs from solver 0 in constraint %d: %s' % (j, i, diff))
     total = solvers[0].model.total
-    keys = [sampler_columns(smp, total) for smp in samplers]
-    if len({key for key, _ in keys}) > 1:
+    if len({sampler_columns(smp, total)[0] for smp in samplers}) > 1:
         return 'the members\' samplers differ in their in-kernel columns, or some sample on the host'
-    cols = keys[0][1]
-    host = keys[0][0] is None
     opts = []
     for eng in engines:
         opt, _ = eng._optimizer_for(optimizer, lr, dict(kwargs))
         if not plain_adam(opt):
             return 'the optimizer is not plain torch.optim.Adam with one parameter group'
         opts.append(opt)
-    hyper = [adam_hyper(o) for o in opts]
-    if len(set(hyper)) > 1:
+    if len({adam_hyper(o) for o in opts}) > 1:
         return 'the members\' Adam hyper-parameters differ'
-    return _run(solvers, engines, opts, terms[0], niters, batch_size, samplers if host else None, cols, k, hyper[0])
+    return run_persistent(engines, opts, samplers, terms[0], niters, batch_size, k, table=True)
 
-
-def _run(solvers, engines, opts, terms, niters, batch_size, host_samplers, cols, k, hyper):
-    """ `niters` steps of every member, `k` per launch, members in launches of at most MAX_MEMBERS.  Returns None, or
-    the reason the kernels refused the first launch (nothing has been trained then). """
-    lr, (b1, b2), eps, wd = hyper
-    e0 = engines[0]
-    lib, total = e0.lib, solvers[0].model.total
-    total_sum = e0._sum_reduction()
-    term_arr = (_native.PinnTerm * max(1, len(terms)))()
-    for i, e in enumerate(terms):
-        term_arr[i].plan = e['plan'].value
-        term_arr[i].n_points = e['n']
-        term_arr[i].point_weight = 1.0 if total_sum else 1.0 / e['n']
-        term_arr[i].points = e['host_points'].data_ptr()
-    point_weight = 1.0 if total_sum else 1.0 / batch_size
-    M = len(solvers)
-    members = (_native.PinnMember * M)()
-    starts, step0 = [], []
-    for j, (s, eng, opt) in enumerate(zip(solvers, engines, opts)):
-        if s.optimizer is not eng._opt_obj:
-            eng._drop_graphs()
-            eng._opt_obj, eng._opt_key = s.optimizer, None
-        mask = eng._bind_adam_state(opt)
-        m, v, steps, _ = eng._adam_flat
-        mb = members[j]
-        mb.params, mb.exp_avg, mb.exp_avg_sq, mb.mask = eng.flat.data_ptr(), m.data_ptr(), v.data_ptr(), mask.data_ptr()
-        mb.step_tensors, mb.n_step_tensors = steps.data_ptr(), steps.numel()
-        mb.seed, mb.step_counter, mb.losses_ring = eng.seed, eng.step_counter.data_ptr(), eng.ring.data_ptr()
-        step0.append(float(steps.max().item()))
-        starts.append(eng.steps_done)
-        s.model.train()
-    ring_len = e0.ring.numel()
-    vals = np.empty((M, niters), dtype=np.float32)
-    stream = e0._stream()
-    size = C.sizeof(_native.PinnMember)
-
-    def drain(upto, drained):
-        torch.cuda.synchronize(e0.device)
-        for j, eng in enumerate(engines):
-            vals[j, drained:upto] = eng.ring.cpu().numpy()[(starts[j] + np.arange(drained, upto)) % ring_len]
-
-    done, drained = 0, 0
-    while done < niters:
-        kk = min(k, niters - done, ring_len)
-        if done + kk - drained > ring_len:
-            drain(done, drained)
-            drained = done
-        batches = []
-        if host_samplers is not None:
-            for j, smp in enumerate(host_samplers):
-                host = torch.empty((kk, batch_size, total), dtype=torch.float32).pin_memory()
-                for i in range(kk):
-                    b = smp.sample(batch_size)
-                    host[i].copy_(b if isinstance(b, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(b, dtype=np.float32)))
-                batches.append(host.to(e0.device, non_blocking=True))
-                members[j].points = batches[-1].data_ptr()
-        for j in range(M):
-            members[j].opt_step0 = step0[j] + done
-        for lo in range(0, M, _native.MAX_MEMBERS):
-            n = min(_native.MAX_MEMBERS, M - lo)
-            rc = lib.pinn_multi_step_ensemble(
-                e0.plan, n, C.cast(C.addressof(members) + lo * size, C.POINTER(_native.PinnMember)),
-                C.c_int64(batch_size), C.c_int(kk), C.c_float(lr), C.c_float(b1), C.c_float(b2), C.c_float(eps),
-                C.c_float(wd), C.c_int64(ring_len), C.c_float(point_weight), C.c_int(len(terms)), term_arr, cols, stream)
-            if rc == _native.E_UNSUPPORTED and done == 0 and lo == 0:
-                return lib.pinn_last_error().decode('utf-8', 'replace')
-            _native.check(rc)
-        done += kk
-    drain(niters, drained)
-    for j, (s, eng) in enumerate(zip(solvers, engines)):
-        eng.steps_done = starts[j] + niters
-        s.losses.extend(np.array(x, dtype=np.float32) for x in vals[j])
-    return None

@@ -29,8 +29,6 @@ try:                                           # progress bar like the reference
 except ImportError:                            # pragma: no cover
     _tqdm = None
 
-_GRAPH_MIN_ITERS = 8
-
 
 def _progress(n):
     if _tqdm is None or os.environ.get('PYDENS_B200_PROGRESS', '') == '0':
