@@ -122,10 +122,21 @@ def sampler_columns(sampler, total):
 
 def plain_adam(opt):
     """ The optimizer is the Adam the kernels implement: torch.optim.Adam, one parameter group, no amsgrad, no
-    maximize, a float lr. """
+    maximize, a float lr, and weight decay added to the gradient (L2).  Adam(decoupled_weight_decay=True) is AdamW,
+    which the kernels do not implement; with zero weight decay both forms are the same update. """
     g = opt.param_groups[0] if opt.param_groups else {}
     return (type(opt) is torch.optim.Adam and len(opt.param_groups) == 1 and not g.get('amsgrad')
-            and not g.get('maximize') and not torch.is_tensor(g.get('lr')))
+            and not g.get('maximize') and not torch.is_tensor(g.get('lr'))
+            and not (g.get('decoupled_weight_decay') and g.get('weight_decay')))
+
+
+def adam_steps_equal(opt):
+    """ Every parameter of the optimizer has taken the same number of steps (a parameter without state: none).  torch
+    keeps one step count per tensor, the kernels take one t for all of them; a state loaded with differing counts runs
+    on torch's Adam. """
+    steps = {float(st['step']) if st and 'step' in st else 0.0
+             for st in (opt.state.get(p) for g in opt.param_groups for p in g['params'])}
+    return len(steps) <= 1
 
 
 def adam_hyper(opt):
@@ -513,9 +524,15 @@ class FusedEngine:
         m, v, steps, mask = self._adam_flat
         in_opt = {id(q) for g in opt.param_groups for q in g['params']}
         sig = (id(opt), tuple(sorted(in_opt)))
+
+        def bound(st, idx, o):
+            # all three state tensors are still the views: load_state_dict keeps a moment that is already on the device
+            # and replaces a step given on the host, so one of them alone says nothing about the others
+            return (st is not None and 'exp_avg' in st and st['exp_avg'].data_ptr() == m.data_ptr() + 4 * o
+                    and st['exp_avg_sq'].data_ptr() == v.data_ptr() + 4 * o and torch.is_tensor(st['step'])
+                    and st['step'].data_ptr() == steps.data_ptr() + 4 * idx)
         if self._adam_bound_to is opt and self._adam_bound_sig == sig and all(
-                (st := opt.state.get(p)) is not None and 'exp_avg' in st and st['exp_avg'].data_ptr() == m.data_ptr() + 4 * o
-                for p, o in self.entries if id(p) in in_opt):
+                bound(opt.state.get(p), idx, o) for idx, (p, o) in enumerate(self.entries) if id(p) in in_opt):
             return mask                                 # same optimizer, same parameters, still bound: nothing to do
         mask.zero_()
         rebound = False
@@ -528,8 +545,8 @@ class FusedEngine:
                 st = opt.state.get(p)
                 mv, vv = m[o:o + n].view(p.shape), v[o:o + n].view(p.shape)
                 if st and 'exp_avg' in st:
-                    if st['exp_avg'].data_ptr() == mv.data_ptr():
-                        continue                                    # already bound
+                    if bound(st, idx, o):
+                        continue
                     mv.copy_(st['exp_avg']); vv.copy_(st['exp_avg_sq']); steps[idx] = float(st['step'])
                 else:
                     mv.zero_(); vv.zero_(); steps[idx] = 0.0
@@ -577,7 +594,7 @@ class FusedEngine:
             steps_per_launch = _AUTO_PERSISTENT_STEPS
         if steps_per_launch > 0 and niters > 0:
             terms = None
-            if plain_adam(opt) and _dist() is None and batch_size > 0:
+            if plain_adam(opt) and adam_steps_equal(opt) and _dist() is None and batch_size > 0:
                 terms = self._persistent_terms(loss_terms, batch_size)
             if terms is not None and self._fit_persistent(niters, batch_size, sampler, opt, steps_per_launch, terms):
                 return
@@ -626,6 +643,7 @@ class FusedEngine:
         # engine builds and nothing has to touch the gradient between the kernel and the update
         capturable = bool(opt.param_groups and opt.param_groups[0].get('capturable', False))
         fused_adam = (os.environ.get('PYDENS_B200_FUSED_ADAM', '1') != '0' and plain_adam(opt) and capturable
+                      and adam_steps_equal(opt)
                       and not fused_constraints and not nums and not stray_params and eq_term
                       and (dist is None or self.comm is not None))
         adam, adam_key = None, None

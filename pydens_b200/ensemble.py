@@ -12,8 +12,8 @@ import warnings
 from torch import nn
 
 from . import _native
-from .engine import (_AUTO_PERSISTENT_STEPS, _dist, adam_hyper, auto_persistent, plain_adam, run_persistent,
-                     sampler_columns)
+from .engine import (_AUTO_PERSISTENT_STEPS, _dist, adam_hyper, adam_steps_equal, auto_persistent, plain_adam,
+                     run_persistent, sampler_columns)
 
 # what each part of the problem's spec describes, for the error that names the difference between two members
 _SPEC_PARTS = (
@@ -72,7 +72,8 @@ def fit_ensemble(solvers, niters, batch_size, sampler=None, loss_terms='equation
               member's batch from its own seed; a shared host sampler gives each member its batches in member order,
               launch by launch.
     Anything the persistent path cannot take fits the solvers one after another with their own `fit`, after one
-    UserWarning giving the reason.  Raises ValueError for the same Solver twice, solvers on different devices, or
+    UserWarning giving the reason; decoupled weight decay (decoupled_weight_decay=True with weight_decay > 0) is one
+    such fit, it runs on torch's Adam.  Raises ValueError for the same Solver twice, solvers on different devices, or
     solvers whose problems differ.
     """
     solvers = list(solvers)
@@ -137,7 +138,10 @@ def _fit_together(solvers, niters, batch_size, samplers, loss_terms, optimizer, 
     for eng in engines:
         opt, _ = eng._optimizer_for(optimizer, lr, dict(kwargs))
         if not plain_adam(opt):
-            return 'the optimizer is not plain torch.optim.Adam with one parameter group'
+            return ('the optimizer is not plain torch.optim.Adam with one parameter group and L2 weight decay '
+                    '(decoupled weight decay runs on torch\'s Adam)')
+        if not adam_steps_equal(opt):
+            return 'the optimizer has taken different numbers of steps for different parameters'
         opts.append(opt)
     if len({adam_hyper(o) for o in opts}) > 1:
         return 'the members\' Adam hyper-parameters differ'

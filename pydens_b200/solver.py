@@ -305,6 +305,9 @@ class Solver:
                     whenever the optimizer is plain Adam, there is one device, the equation is a loss term and every
                     constraint term runs fused (at most 4 of them, 32 constraint points in all)
                     (PYDENS_B200_AUTO_PERSISTENT=0 keeps one launch per step).
+                    Decoupled weight decay (decoupled_weight_decay=True with weight_decay > 0, or optimizer='AdamW')
+                    trains one step at a time with torch's Adam after the step kernel, and so does an optimizer state
+                    whose parameters have taken different numbers of steps.
         """
         loss_terms = loss_terms if isinstance(loss_terms, (tuple, list)) else (loss_terms,)
         ok, why = self._fused_possible(criterion, loss_terms)

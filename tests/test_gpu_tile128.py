@@ -390,13 +390,15 @@ class _AdamState:
         return c
 
 
-def _step_adam(p, st, pts):
+def _step_adam(p, st, pts, hyper=ADAM, ring=None):
+    """ pinn_step_adam on explicit points with the hyper-parameters `hyper`; `ring`: the device loss ring, or None """
     n = pts.shape[0]
     need = int(p.lib.pinn_workspace_bytes(p.plan, n))
     if p.ws is None or p.ws.numel() < need:
         p.ws = torch.zeros(need, dtype=torch.uint8, device=p.dev)
     adam = N.PinnAdam(st.m.data_ptr(), st.v.data_ptr(), st.mask.data_ptr(), st.steps.data_ptr(), st.steps.numel(),
-                      ADAM['lr'], ADAM['beta1'], ADAM['beta2'], ADAM['eps'], ADAM['weight_decay'], None, 0)
+                      hyper['lr'], hyper['beta1'], hyper['beta2'], hyper['eps'], hyper['weight_decay'],
+                      ring.data_ptr() if ring is not None else None, ring.numel() if ring is not None else 0)
     N.check(p.lib.pinn_step_adam(p.plan, None, C.c_void_p(st.p.data_ptr()), C.c_void_p(pts.data_ptr()), None,
                                  C.c_uint64(0), C.c_void_p(st.counter.data_ptr()), C.c_uint64(0), C.c_int64(n),
                                  C.c_float(1.0 / n), C.c_void_p(st.out.data_ptr()), None, C.c_void_p(p.ws.data_ptr()),
