@@ -1267,12 +1267,15 @@ PINN_HD int term_of(const DevTerms& T, int i) {
 // leaves dr/d(that channel) in slot eq_out[1] + j*C + c.
 // TERMS (one output): a point of a constraint term when `term` is set — the same forward jets, its own residual program
 // on the value channel, weight term->weight, zero adjoint seeds on the derivative channels (term_seeds).
-template <int NF, int NS, int JF, bool GEN = true, bool MULTI = false, bool TERMS = false>
+// REMAT0: the plan has the compact layout of build_remat_plan — the first layer's jet is rebuilt for the reverse pass
+// instead of kept, and the output layer's adjoint and the dump rows sit in the scratch rows.
+template <int NF, int NS, int JF, bool GEN = true, bool MULTI = false, bool TERMS = false, bool REMAT0 = false>
 PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weights */,
                          const float* __restrict__ pvals /* flat params (for log_scale, V) */,
                          float* __restrict__ st, int RS, bool valid, float inv_n,
                          const GradSink& sink, PointPartials<NF, NS>& part, const DevTerm* term = nullptr) {
     static_assert(!(TERMS && MULTI), "constraint terms: networks of one output");
+    static_assert(!(REMAT0 && (MULTI || TERMS)), "the compact layout: networks of one output, no constraint terms");
     constexpr int C = 1 + NF + NS;
     const int Ln = P.n_layers;
     float* coords = st;
@@ -1312,7 +1315,8 @@ PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weigh
     float log_scale = pvals[P.log_scale_off];
     AnsatzState<NF, NS> as;
     float u[C];
-    float* top_rows = units + (size_t)P.layer[Ln - 1].unit_base * C * RS;
+    float* top_rows = REMAT0 ? scr : units + (size_t)P.layer[Ln - 1].unit_base * C * RS;
+    float* dump_rows = REMAT0 ? scr + (size_t)C * RS : scr;
     const int n_out = MULTI ? P.layer[Ln - 1].n_out : 1;
     if constexpr (MULTI) {
 #pragma unroll 1
@@ -1388,9 +1392,11 @@ PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weigh
     for (int l = Ln - 1; l >= 1; --l) {
         PINN_PHASE_T0(t_rev);
         const DevLayer& L = P.layer[l];
-        float* out_rows = units + (size_t)L.unit_base * C * RS;
+        float* out_rows = (REMAT0 && l == Ln - 1) ? top_rows : units + (size_t)L.unit_base * C * RS;
         const DevLayer& B = P.layer[l - 1];                 // the layer below
         float* in_rows = units + (size_t)B.unit_base * C * RS;
+        if (REMAT0 && l == 1)                               // the first layer's jet again, behind layer 1's adjoint
+            fwd_layer<NF, NS, JF, GEN>(B, sw, coords, true, PINN_ACT_NONE, &P.dir_vec[0][0], in_rows, RS);
         int load_act;
         const float* load_rows = layer_output<GEN>(P, l - 1, units, C, RS, load_act);
         const float* adj_in = B.adj_from >= 0 ? units + (size_t)P.layer[B.adj_from].post_base * C * RS : nullptr;
@@ -1399,8 +1405,8 @@ PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weigh
             if (L.n_out == 1) bwd_layer<NF, NS, 1, true>(L, B.act, sw, out_rows, in_rows, RS, sink, load_rows, load_act, adj_in, adj_out, scr);
             else              bwd_layer<NF, NS, 4, true>(L, B.act, sw, out_rows, in_rows, RS, sink, load_rows, load_act, adj_in, adj_out, scr);
         } else {
-            if (L.n_out == 1) bwd_layer<NF, NS, 1, false, GEN>(L, B.act, sw, out_rows, in_rows, RS, sink, in_rows, B.act, nullptr, nullptr, scr);
-            else              bwd_layer<NF, NS, 4, false, GEN>(L, B.act, sw, out_rows, in_rows, RS, sink, in_rows, B.act, nullptr, nullptr, scr);
+            if (L.n_out == 1) bwd_layer<NF, NS, 1, false, GEN>(L, B.act, sw, out_rows, in_rows, RS, sink, in_rows, B.act, nullptr, nullptr, dump_rows);
+            else              bwd_layer<NF, NS, 4, false, GEN>(L, B.act, sw, out_rows, in_rows, RS, sink, in_rows, B.act, nullptr, nullptr, dump_rows);
         }
         PINN_PHASE_ADD(PINN_PHASE_REV + l, t_rev);
     }

@@ -175,6 +175,30 @@ inline int build_dev_plan(const PinnSpec* s, DevPlan& h, int& fwd_rows, int& fwd
     return PINN_OK;
 }
 
+// The step kernel's compact per-point layout (point_step<…, REMAT0 = true>), for plain one-output networks of two hidden
+// layers or more.  The first layer's jet is never kept: its first-order channels are the same for every point and its
+// second-order ones vanish, and its values cost one tiny layer over the coordinates, so the forward pass builds it in rows
+// that the second hidden layer takes over later, and the reverse pass rebuilds it, bit for bit, in the same rows once
+// that layer's adjoint is spent.  The output layer's adjoint and the rows that swallow masked-off stores share the
+// program's scratch rows, which are dead by then.  Per point: the coordinates, hidden layers 1 .. n-2 (at least as many
+// rows as layers 0 and 1 take together), and max(n_slots, 2 C) scratch rows — cfg2 ([2, 10, 12, 15, 1], C = 5): 147 rows
+// instead of 200.
+// Fills `c` from the plan `h` and returns true, or returns false where the compact layout does not apply.
+inline bool build_remat_plan(const DevPlan& h, DevPlan& c) {
+    const int Ln = h.n_layers;
+    if (h.general || Ln < 3 || h.layer[Ln - 1].n_out != 1) return false;
+    const int C = 1 + h.nf + h.ns;
+    c = h;
+    int units = 0;
+    for (int l = 1; l < Ln - 1; ++l) { c.layer[l].unit_base = units; units += h.layer[l].n_out; }
+    c.layer[0].unit_base = h.layer[1].n_out;                  // behind layer 1 (over layer 2's rows, if that is hidden)
+    c.layer[Ln - 1].unit_base = 0;                            // unused: the output layer's adjoint lives in the scratch rows
+    const int first_end = h.layer[1].n_out + h.layer[0].n_out;
+    c.row_scr = h.total + C * (units > first_end ? units : first_end);
+    c.rows_total = c.row_scr + (h.n_slots > 2 * C ? h.n_slots : 2 * C);
+    return true;
+}
+
 // Re-layout of the flat parameters into the weight area (what stage_plan_and_weights does on the GPU).
 inline void host_stage_weights(const DevPlan& P, const float* params, float* sw) {
     for (int i = 0; i < P.weights_floats; ++i) sw[i] = 0.0f;

@@ -40,6 +40,8 @@ void enter() {
     if constexpr (GEN) {
         k.multi = multi_step_kernel<NF, J, Cfg::MAXT, Cfg::JF>;
         k.multi_ensemble = multi_step_ensemble_kernel<NF, J, Cfg::MAXT, Cfg::JF>;
+    } else if constexpr (NF == 2 && J == 2) {
+        k.step_w12 = step_kernel_w12<NF, J, Cfg::JF>;
     }
     k.maxt = Cfg::MAXT;
 #elif PINN_UNIT == PINN_STEP_GMEM

@@ -174,7 +174,10 @@ struct PinnPlan {
     int multi_budget, small_budget;          // dynamic shared memory the two can take (constraint programs with more slots)
     int wide_ctas;                           // CTAs the tile kernel runs on (<= sm_count)
     const KernelSet* ks;                     // the kernels of this plan's jet set
-    StepKernelFn fn_smem, fn_gmem;           // the pair matching this plan (plain or general, or coupled_step_kernel)
+    StepKernelFn fn_smem, fn_gmem;           // the pair matching this plan (plain or general, or coupled_step_kernel);
+                                             // fn_smem is step_kernel_w12 when the twelve-warp form was placed
+    DevPlan hs;                              // the plan the thread step kernel runs on: h, or its compact layout
+                                             // (build_remat_plan) under step_kernel_w12
     bool coupled;                            // a network of 2..4 outputs: coupled_step_kernel / coupled_forward_kernel,
                                              // or the coupled form of the 128-wide tile kernel
     int sm_count;
@@ -240,6 +243,27 @@ static int place_step_kernel(PinnPlan* p) {
     if (force && !strcmp(force, "smem") && best_nw >= 1) use_smem = true;
     if (force && !strcmp(force, "gmem")) use_smem = false;
     if (!has_smem_form) use_smem = false;
+    // three warps per scheduler: the twelve-warp form on the compact per-point layout, where its 384 threads fit (register
+    // count, and the storage of twelve warps with their accumulators in shared memory or else in the workspace) and
+    // outnumber the warps placed above (cfg2: 12 instead of 8)
+    DevPlan hc;
+    const StepKernelFn f12 = p->coupled ? nullptr : p->ks->step_w12;
+    if (f12 && !(force && !strcmp(force, "gmem")) && build_remat_plan(h, hc) && (!use_smem || best_nw < 12)) {
+        cudaFuncAttributes f12a;
+        e = cudaFuncGetAttributes(&f12a, (const void*)f12);
+        if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncGetAttributes: %s", cudaGetErrorString(e));
+        const int budget12 = p->smem_optin - (int)f12a.sharedSizeBytes - 64;
+        for (int pass = 0; pass < 2 && max_warps(f12a, 384) == 12; ++pass) {
+            const int nwacc = pass == 0 ? 12 : 0;
+            const SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, nwacc, storage_floats(hc, hc.rows_total, 12));
+            if (SL.total_f * 4 > budget12) continue;
+            p->fn_smem = f12; p->hs = hc; p->regs = f12a.numRegs;
+            p->gmem = false; p->threads = 384; p->wacc_gmem = nwacc == 0; p->smem_bytes = SL.total_f * 4;
+            e = allow_max_smem((const void*)f12, p->smem_optin);
+            if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(smem=%d): %s", p->smem_bytes, cudaGetErrorString(e));
+            return PINN_OK;
+        }
+    }
     if (use_smem) {
         p->gmem = false; p->threads = best_nw * 32; p->wacc_gmem = best_nwacc == 0;
         SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, best_nwacc, storage_floats(h, h.rows_total, best_nw));
@@ -372,7 +396,7 @@ static int place_wide_kernel(PinnPlan* p, int order, int thread_rc) {
     e = cudaFuncGetAttributes(&fa, (const void*)f);
     if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncGetAttributes(wide): %s", cudaGetErrorString(e));
     p->fn_wide = f;
-    p->wide = true; p->wide_kw = kw; p->gmem = true; p->threads = wide::NT; p->wacc_gmem = false;
+    p->wide = true; p->wide_kw = kw; p->gmem = true; p->threads = wide::NT; p->wacc_gmem = false; p->hs = p->h;
     p->smem_bytes = smem; p->regs = fa.numRegs;
     if (thread_rc != PINN_OK) {                 // the forward kernel does not hold this network either
         const void* ff = p->coupled ? (const void*)wide::wide128_coupled_forward_kernel : (const void*)wide::wide128_forward_kernel;
@@ -413,6 +437,7 @@ extern "C" int pinn_plan_create(const PinnSpec* s, int device, PinnPlan** out) {
     }
     p->spec = *s;
     p->device = device;
+    p->hs = p->h;
 
     cudaError_t e = cudaSetDevice(device);
     if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaSetDevice(%d): %s", device, cudaGetErrorString(e));
@@ -698,7 +723,7 @@ static int step_impl(const PinnPlan* cp, const PinnComm* comm, const float* para
     if (comm && (!comm->connected || comm->bytes != comm_bytes(p->h.n_params + 4, comm->world)))
         return fail(PINN_E_INVALID, "communicator is not connected or belongs to another plan");
     cudaStream_t st = (cudaStream_t)stream;
-    DevPlan plan = p->h;
+    DevPlan plan = p->hs;
     if (!points) { int rc = resolve_cols(p, cols, plan.cols); if (rc) return rc; }
     StepArgs a;
     a.params = params; a.points = points; a.seed = seed;
@@ -708,7 +733,7 @@ static int step_impl(const PinnPlan* cp, const PinnComm* comm, const float* para
     a.partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_partials_off());
     a.spill = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_spill_off(p));
     a.wacc = ws_wacc_bytes(p) ? reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_wacc_off(p)) : nullptr;
-    a.rows_total = p->h.rows_total;
+    a.rows_total = p->hs.rows_total;
     a.adam_m = nullptr; a.adam_v = nullptr; a.adam_mask = nullptr; a.adam_steps = nullptr; a.adam_n_steps = 0;
     a.adam_lr = a.adam_beta1 = a.adam_beta2 = a.adam_eps = a.adam_wd = 0.0f;
     a.ring = nullptr; a.ring_len = 1;
@@ -1033,7 +1058,7 @@ extern "C" int pinn_plan_info(const PinnPlan* p, PinnPlanInfo* info) {
     info->tensor_core = p->wide ? (p->wide_kw == 128 ? 2 : 1) : 0;
     info->small_batch_points = p->fn_small ? 8 * pinn::small::BP : 0;
     info->smem_bytes = p->smem_bytes; info->regs_per_thread = p->regs; info->sm_count = p->sm_count;
-    info->rows_per_point = p->h.rows_total;
+    info->rows_per_point = p->hs.rows_total;
     info->flops_per_point = 6ll * C * macs;
     info->bytes_per_point = 4 * p->h.total;
     return PINN_OK;

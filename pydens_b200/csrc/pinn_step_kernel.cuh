@@ -425,8 +425,10 @@ __device__ __forceinline__ void cta_partial(const StepArgs& a, const float* wacc
 // ---------------------------------------------------------------------------------------------------
 // The fit-step kernel.
 // ---------------------------------------------------------------------------------------------------
-// The body of every thread-kernel step: MULTI selects the form for networks of 2..4 outputs (point_step).
-template <int NF, int NS, bool GMEM, int JF, bool GEN, bool MULTI>
+// The body of every thread-kernel step: MULTI selects the form for networks of 2..4 outputs, REMAT0 the compact per-point
+// layout (point_step).  PF: coordinate columns of the next tile prefetched into registers; the columns past PF are loaded
+// when the tile starts.
+template <int NF, int NS, bool GMEM, int JF, bool GEN, bool MULTI, bool REMAT0 = false, int PF = PINN_MAX_DIMS>
 __device__ __forceinline__ void step_body(const DevPlan& P, const StepArgs& a) {
     extern __shared__ __align__(16) float smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
@@ -455,12 +457,15 @@ __device__ __forceinline__ void step_body(const DevPlan& P, const StepArgs& a) {
 
     // explicit batches: the coordinates of this warp's next tile are loaded into registers while the current tile runs
     // (the batch pool is larger than L2, so each load would otherwise stall the warp for a trip to HBM)
-    float next_pt[PINN_MAX_DIMS];
-    auto load_tile = [&](long long tile) {
+    float next_pt[PF];
+    auto tile_src = [&](long long tile) {
         const long long pl = tile * 32 + lane;
-        const float* src = a.points + (size_t)(pl < a.n_points ? pl : a.n_points - 1) * P.total;
+        return a.points + (size_t)(pl < a.n_points ? pl : a.n_points - 1) * P.total;
+    };
+    auto load_tile = [&](long long tile) {
+        const float* src = tile_src(tile);
 #pragma unroll
-        for (int k = 0; k < PINN_MAX_DIMS; ++k)
+        for (int k = 0; k < PF; ++k)
             if (k < P.total) next_pt[k] = __ldg(src + k);
     };
     // tiles are dealt warp-slot-major (slot w of every CTA before slot w+1 of any): the last, partial round of tiles
@@ -474,8 +479,12 @@ __device__ __forceinline__ void step_body(const DevPlan& P, const StepArgs& a) {
         const long long pe = valid ? pl : a.n_points - 1;     // masked lanes replay the last point
         if (a.points) {
 #pragma unroll
-            for (int k = 0; k < PINN_MAX_DIMS; ++k)
+            for (int k = 0; k < PF; ++k)
                 if (k < P.total) st[k * RS] = next_pt[k];
+            if (PF < PINN_MAX_DIMS) {
+                const float* src = tile_src(tile);
+                for (int k = PF; k < P.total; ++k) st[k * RS] = __ldg(src + k);
+            }
             if (tile + total_warps < n_tiles) load_tile(tile + total_warps);
         } else {
             const uint64_t gidx = a.point_offset + (uint64_t)pe;
@@ -485,7 +494,7 @@ __device__ __forceinline__ void step_body(const DevPlan& P, const StepArgs& a) {
             for (int k = 0; k < P.total; ++k) st[k * RS] = sample_column(P.cols[k], k, gidx, step, a.seed, b0, b1);
         }
         PINN_PHASE_ADD(PINN_PHASE_LOAD, t_load);
-        float r = point_step<NF, NS, JF, GEN, MULTI>(P, sw, a.params, st, RS, valid, a.inv_n, sink, part);
+        float r = point_step<NF, NS, JF, GEN, MULTI, false, REMAT0>(P, sw, a.params, st, RS, valid, a.inv_n, sink, part);
         if (a.residual && valid) a.residual[pl] = r;
     }
 
@@ -515,6 +524,13 @@ __device__ __forceinline__ void step_body(const DevPlan& P, const StepArgs& a) {
 template <int NF, int NS, bool GMEM, int MAXT, int JF, bool GEN>
 __global__ void __launch_bounds__(MAXT, 1) step_kernel(const __grid_constant__ DevPlan P, const StepArgs a) {
     step_body<NF, NS, GMEM, JF, GEN, false>(P, a);
+}
+
+// The twelve-warp form (three warps per scheduler) of a plain step on the compact layout (build_remat_plan): 384 threads
+// leave 168 registers per thread, which the next tile's coordinates fit only up to four columns.
+template <int NF, int NS, int JF>
+__global__ void __launch_bounds__(384, 1) step_kernel_w12(const __grid_constant__ DevPlan P, const StepArgs a) {
+    step_body<NF, NS, false, JF, false, false, true, 4>(P, a);
 }
 
 // The step of a network with 2..4 outputs (coupled systems): the general form, k read from the plan at run time.
@@ -719,6 +735,7 @@ struct KernelSet {
     StepKernelFn coupled_wide128;            // the coupled form of the 128-wide tile kernel
     EnsembleKernelFn multi_ensemble;         // the ensemble forms of `multi` and `small` (null where those are)
     EnsembleKernelFn small_ensemble;
+    StepKernelFn step_w12;                   // step_kernel_w12 (nf = ns = 2 only; null elsewhere)
 };
 
 // The set of a jet set, or nullptr when none was built: 0 <= ns <= nf <= PINN_MAX_DIRS for order 2; 1 <= nf <= 4 and
