@@ -368,9 +368,12 @@ int pinn_step_adam(const PinnPlan* plan, const PinnComm* comm_or_null, float* pa
  * pinn_multi_step_terms: the same with constraint terms (reference :451-457, `loss_terms=['equation', 'constraint_0']`).
  * One optimizer step is the gradient of  point_weight * sum_batch r^2  +  sum_k term_k.point_weight * sum_{its points} r_k^2,
  * and the logged loss is that sum.  point_weight is 1 / n_points for a mean criterion, 1 for reduction='sum'.
- * A term is a constraint plan (pinn_plan_create on a spec with no derivative directions whose residual program is the
- * constraint, evaluated on u at fixed points) with the same layer table, n_params and log_scale_off as `plan`, the same
- * ansatz, and variables among the plan's.  Its points are read from HOST memory during the call and travel to the
+ * A term is a constraint plan (pinn_plan_create on a spec whose residual program is the constraint, evaluated on the
+ * jet of u at fixed points) with the same layer table, n_params and log_scale_off as `plan`, the same ansatz, and
+ * variables among the plan's.  Its jet set is either empty (nf = ns = 0: the program reads u alone, C = 1) or exactly
+ * the plan's (the same nf, ns, dir_vec and order 2: it reads every channel c of the plan's jet in slot c, and its
+ * eq_out holds dr/d(channel c) for all C channels, as an equation program's does) — a constraint such as u'(0) = 0
+ * differentiates u at its points through the jets the kernel already carries.  Its points are read from HOST memory during the call and travel to the
  * kernel by value, with the residual program: the call allocates nothing and stays stream-ordered and capturable.
  * They do not consume sampler counters: an in-kernel batch is the one pinn_sample gives.  At most PINN_MAX_TERMS terms
  * and PINN_MAX_TERM_POINTS points in all; n_points + the term points <= pinn_multi_step_max_points.  A term plan that

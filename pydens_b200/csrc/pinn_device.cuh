@@ -118,17 +118,19 @@ struct alignas(16) DevPlan {
     PinnInstr ic[PINN_MAX_PROG];
 };
 
-// A constraint term of the persistent multi-step kernels (pinn_multi_step_terms): its residual program runs on u (the
-// value channel of the equation's ansatz) at fixed points.  Its slots are the constraint plan's: slot 0 holds u,
-// eq_out = [r, dr/du, dr/dV_i ..], and PINN_OP_VAR operands index ITS variable list (var_off: flat offsets);
-// var_map[i] is the equation variable with the same offset, whose partial it adds to.
+// A constraint term of the persistent multi-step kernels (pinn_multi_step_terms): its residual program runs on the jet
+// of u (the equation's ansatz) at fixed points.  Its slots are the constraint plan's: slots 0 .. C-1 hold the channels
+// its program reads — C = 1, the value alone, or the equation's whole jet set —, eq_out = [r, dr/dchannel_c (C), dr/dV_i
+// ..], and PINN_OP_VAR operands index ITS variable list (var_off: flat offsets); var_map[i] is the equation variable
+// with the same offset, whose partial it adds to.
 struct DevTerm {
     int n_eq;
     float weight;                       // the term's point weight: 1 / n (mean) or 1 (sum)
     int var_off[PINN_MAX_VARS];
     int var_map[PINN_MAX_VARS];
     int n_vars;
-    int eq_out[2 + PINN_MAX_VARS];
+    int C;                              // jet channels of its program: 1, or the plan's 1 + nf + ns
+    int eq_out[1 + 1 + 2 * PINN_MAX_DIRS + PINN_MAX_VARS];
     PinnInstr eq[PINN_MAX_PROG];
 };
 struct DevTerms {
@@ -1227,30 +1229,37 @@ PINN_HD void ic_var_partials(const DevPlan& P, const float* __restrict__ scr, in
     }
 }
 
-// A constraint term's point (DevTerm): the initial condition's d(ic)/dV_i of the value channel, read BEFORE the term's
-// program runs — that program's slots are the constraint plan's and may cover the equation plan's ic_out slots.
-template <int NF, int NS>
-PINN_HD void term_ic_partials(const DevPlan& P, const float* __restrict__ scr, int RS, float (&icv)[PINN_MAX_VARS]) {
-    constexpr int C = 1 + NF + NS;
-#pragma unroll
-    for (int i = 0; i < PINN_MAX_VARS; ++i)
-        icv[i] = (P.ic_has_vars && i < P.n_vars) ? scr[(size_t)P.ic_out[C * (1 + i)] * RS] : 0.0f;
-}
-// ... and, after it ran (rb = 2 r weight), the adjoint seeds of the jet — the value channel only — and the partials of the
-// equation's variables: dr/dV of the term's variables that share their offset, plus the initial condition's share.
+// A constraint term's point (DevTerm), after its program ran (rb = 2 r weight): the adjoint seeds of the jet — the
+// term's C channels, zero on the others — and the partials of the equation's variables: dr/dV of the term's variables
+// that share their offset.
 template <int NF, int NS>
 PINN_HD void term_seeds(const DevPlan& P, const DevTerm& T, const float* __restrict__ scr, int RS, float rb,
-                        const float (&icv)[PINN_MAX_VARS], float (&ub)[1 + NF + NS], PointPartials<NF, NS>& part) {
+                        float (&ub)[1 + NF + NS], PointPartials<NF, NS>& part) {
     constexpr int C = 1 + NF + NS;
-    ub[0] = rb * scr[(size_t)T.eq_out[1] * RS];
 #pragma unroll
-    for (int c = 1; c < C; ++c) ub[c] = 0.0f;
+    for (int c = 0; c < C; ++c) ub[c] = c < T.C ? rb * scr[(size_t)T.eq_out[1 + c] * RS] : 0.0f;
 #pragma unroll
     for (int j = 0; j < PINN_MAX_VARS; ++j) {
         if (j < P.n_vars) {
             for (int i = 0; i < T.n_vars; ++i)
-                if (T.var_map[i] == j) part.vbar[j] = fmaf(rb, scr[(size_t)T.eq_out[2 + i] * RS], part.vbar[j]);
-            if (P.ic_has_vars) part.vbar[j] = fmaf(ub[0], icv[j], part.vbar[j]);
+                if (T.var_map[i] == j) part.vbar[j] = fmaf(rb, scr[(size_t)T.eq_out[1 + T.C + i] * RS], part.vbar[j]);
+        }
+    }
+}
+// ... then the initial condition's share, sum_c ub_c d(ic channel c)/dV_j over the term's channels.  The term's program
+// may have overwritten the equation plan's ic_out slots, so the caller evaluates the plan's ic program again first:
+// at most 32 term points a step pay for that, where reading the C x n_vars partials before the program would keep them
+// in registers across it at every point.
+template <int NF, int NS>
+PINN_HD void term_ic_partials(const DevPlan& P, const DevTerm& T, const float* __restrict__ scr, int RS,
+                              const float (&ub)[1 + NF + NS], PointPartials<NF, NS>& part) {
+    constexpr int C = 1 + NF + NS;
+#pragma unroll
+    for (int j = 0; j < PINN_MAX_VARS; ++j) {
+        if (j < P.n_vars) {
+#pragma unroll
+            for (int c = 0; c < C; ++c)
+                if (c < T.C) part.vbar[j] = fmaf(ub[c], scr[(size_t)P.ic_out[C * (1 + j) + c] * RS], part.vbar[j]);
         }
     }
 }
@@ -1266,7 +1275,7 @@ PINN_HD int term_of(const DevTerms& T, int i) {
 // the shared boundary factor and time gate; the residual program finds channel c of component j in slot j*C + c and
 // leaves dr/d(that channel) in slot eq_out[1] + j*C + c.
 // TERMS (one output): a point of a constraint term when `term` is set — the same forward jets, its own residual program
-// on the value channel, weight term->weight, zero adjoint seeds on the derivative channels (term_seeds).
+// on the term's channels of the jet, weight term->weight, zero adjoint seeds on the other channels (term_seeds).
 // REMAT0: the plan has the compact layout of build_remat_plan — the first layer's jet is rebuilt for the reverse pass
 // instead of kept, and the output layer's adjoint and the dump rows sit in the scratch rows.
 template <int NF, int NS, int JF, bool GEN = true, bool MULTI = false, bool TERMS = false, bool REMAT0 = false>
@@ -1332,10 +1341,8 @@ PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weigh
 #pragma unroll
         for (int c = 0; c < C; ++c) scr[(size_t)c * RS] = u[c];
     }
-    float icv[PINN_MAX_VARS];
     float r;
     if (TERMS && term) {
-        term_ic_partials<NF, NS>(P, scr, RS, icv);
         eval_prog(term->eq, term->n_eq, scr, RS, coords, pvals, term->var_off);
         r = scr[(size_t)term->eq_out[0] * RS];
         inv_n = term->weight;
@@ -1347,7 +1354,11 @@ PINN_HD float point_step(const DevPlan& P, const float* __restrict__ sw /* weigh
     if (valid) part.loss = fmaf(r * inv_n, r, part.loss);
     if (TERMS && term) {
         float ub[C];
-        term_seeds<NF, NS>(P, *term, scr, RS, rb, icv, ub, part);
+        term_seeds<NF, NS>(P, *term, scr, RS, rb, ub, part);
+        if (P.ic_has_vars) {
+            eval_prog(P.ic, P.n_ic, scr, RS, coords, pvals, P.var_off);
+            term_ic_partials<NF, NS>(P, *term, scr, RS, ub, part);
+        }
         float Nb[C];
         part.sbar += ansatz_adjoint<NF, NS>(P, as, ub, Nb);
 #pragma unroll

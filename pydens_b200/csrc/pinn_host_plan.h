@@ -215,4 +215,35 @@ inline void host_stage_weights(const DevPlan& P, const float* params, float* sw)
     }
 }
 
+// A constraint term's plan `g` (spec order `g_order`) next to the plan `h` it trains with: the same network, parameter
+// layout and ansatz, variables among h's, and a jet set the kernels run its program on — no derivative directions
+// (C = 1), or exactly h's (nf, ns, directions, order 2).  Fills `t` (var_map: h's variable of every term variable).
+inline int build_dev_term(const DevPlan& h, int h_order, const DevPlan& g, int g_order, DevTerm& t, char* msg,
+                          size_t msg_len) {
+    if (g.n_layers != h.n_layers || memcmp(g.layer, h.layer, sizeof(DevLayer) * h.n_layers) != 0)
+        PINN_PLAN_FAIL(PINN_E_INVALID, "constraint term: its layer table differs from the plan's");
+    if (g.n_params != h.n_params || g.log_scale_off != h.log_scale_off)
+        PINN_PLAN_FAIL(PINN_E_INVALID, "constraint term: n_params / log_scale_off differ from the plan's");
+    const bool value_only = g.nf == 0 && g.ns == 0 && g_order == 2;
+    const bool same_jets = g.nf == h.nf && g.ns == h.ns && g_order == 2 && h_order == 2 &&
+                           memcmp(g.dir_vec, h.dir_vec, sizeof(h.dir_vec[0]) * h.nf) == 0;
+    if (!value_only && !same_jets)
+        PINN_PLAN_FAIL(PINN_E_INVALID, "constraint term: its plan carries derivative directions other than the plan's");
+    if (g.total != h.total || g.nsp != h.nsp || g.has_bc != h.has_bc || g.has_ic != h.has_ic || g.bc != h.bc ||
+        g.t0 != h.t0 || memcmp(g.lo, h.lo, sizeof(h.lo)) != 0 || memcmp(g.hi, h.hi, sizeof(h.hi)) != 0)
+        PINN_PLAN_FAIL(PINN_E_INVALID, "constraint term: its ansatz differs from the plan's");
+    memset(&t, 0, sizeof(t));
+    t.n_eq = g.n_eq; t.n_vars = g.n_vars;
+    t.C = 1 + g.nf + g.ns;
+    for (int i = 0; i < g.n_vars; ++i) {
+        t.var_off[i] = g.var_off[i];
+        t.var_map[i] = -1;
+        for (int j = 0; j < h.n_vars; ++j) if (h.var_off[j] == g.var_off[i]) t.var_map[i] = j;
+        if (t.var_map[i] < 0) PINN_PLAN_FAIL(PINN_E_INVALID, "constraint term: variable %d is not one of the plan's", i);
+    }
+    for (int i = 0; i < 1 + t.C + g.n_vars; ++i) t.eq_out[i] = g.eq_out[i];     // r, dr/dchannel_c, dr/dV_i
+    memcpy(t.eq, g.eq, sizeof(t.eq));
+    return PINN_OK;
+}
+
 }  // namespace pinn

@@ -804,31 +804,11 @@ extern "C" int pinn_multi_step_max_points(const PinnPlan* p) {
     return (p && p->fn_multi) ? 4096 : ((p && p->fn_small) ? 8 * pinn::small::BP : 0);
 }
 
-// A constraint term's plan next to the plan it trains with: the same network, parameter layout and ansatz, no
-// derivative channels, variables among the plan's.  Fills `t` (var_map: the plan's variable of every term variable).
+// A constraint term's plan next to the plan it trains with (build_dev_term).
 static int term_matches(const PinnPlan* p, const PinnPlan* q, DevTerm& t) {
-    const DevPlan& h = p->h;
-    const DevPlan& g = q->h;
-    if (g.n_layers != h.n_layers || memcmp(g.layer, h.layer, sizeof(DevLayer) * h.n_layers) != 0)
-        return fail(PINN_E_INVALID, "constraint term: its layer table differs from the plan's");
-    if (g.n_params != h.n_params || g.log_scale_off != h.log_scale_off)
-        return fail(PINN_E_INVALID, "constraint term: n_params / log_scale_off differ from the plan's");
-    if (g.nf != 0 || g.ns != 0 || spec_order(&q->spec) != 2)
-        return fail(PINN_E_INVALID, "constraint term: its plan carries derivative directions");
-    if (g.total != h.total || g.nsp != h.nsp || g.has_bc != h.has_bc || g.has_ic != h.has_ic || g.bc != h.bc ||
-        g.t0 != h.t0 || memcmp(g.lo, h.lo, sizeof(h.lo)) != 0 || memcmp(g.hi, h.hi, sizeof(h.hi)) != 0)
-        return fail(PINN_E_INVALID, "constraint term: its ansatz differs from the plan's");
-    memset(&t, 0, sizeof(t));
-    t.n_eq = g.n_eq; t.n_vars = g.n_vars;
-    for (int i = 0; i < g.n_vars; ++i) {
-        t.var_off[i] = g.var_off[i];
-        t.var_map[i] = -1;
-        for (int j = 0; j < h.n_vars; ++j) if (h.var_off[j] == g.var_off[i]) t.var_map[i] = j;
-        if (t.var_map[i] < 0) return fail(PINN_E_INVALID, "constraint term: variable %d is not one of the plan's", i);
-    }
-    for (int i = 0; i < 2 + g.n_vars; ++i) t.eq_out[i] = g.eq_out[i];     // C = 1: r, dr/du, dr/dV_i
-    memcpy(t.eq, g.eq, sizeof(t.eq));
-    return PINN_OK;
+    char msg[256];
+    const int rc = build_dev_term(p->h, spec_order(&p->spec), q->h, spec_order(&q->spec), t, msg, sizeof(msg));
+    return rc ? fail(rc, "%s", msg) : PINN_OK;
 }
 
 // What pinn_multi_step_terms and pinn_multi_step_ensemble share: the checks of the shared arguments and the terms, the

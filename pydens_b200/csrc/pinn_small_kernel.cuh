@@ -200,9 +200,9 @@ __device__ __forceinline__ void small_step_body(const DevPlan& P, const MultiArg
             ansatz_forward<NF, NS, true>(P, coords, SR, flat[P.log_scale_off], N, icj, as, u);
             float ub[C];
             if (term) {
-                float icv[PINN_MAX_VARS];
-                term_ic_partials<NF, NS>(P, sc, SR, icv);
-                sc[0] = u[0];
+#pragma unroll
+                for (int c = 0; c < C; ++c)
+                    if (c < term->C) sc[(size_t)c * SR] = u[c];         // the channels its program reads
                 eval_prog(term->eq, term->n_eq, sc, SR, coords, flat, term->var_off);
                 const float r = sc[(size_t)term->eq_out[0] * SR];
                 const float rb = valid ? 2.0f * r * term->weight : 0.0f;
@@ -210,7 +210,11 @@ __device__ __forceinline__ void small_step_body(const DevPlan& P, const MultiArg
                 PointPartials<NF, NS> part;
 #pragma unroll
                 for (int i = 0; i < PINN_MAX_VARS; ++i) part.vbar[i] = 0.0f;
-                term_seeds<NF, NS>(P, *term, sc, SR, rb, icv, ub, part);
+                term_seeds<NF, NS>(P, *term, sc, SR, rb, ub, part);
+                if (P.ic_has_vars) {
+                    eval_prog(P.ic, P.n_ic, sc, SR, coords, flat, P.var_off);
+                    term_ic_partials<NF, NS>(P, *term, sc, SR, ub, part);
+                }
 #pragma unroll
                 for (int i = 0; i < PINN_MAX_VARS; ++i) red[(2 + i) * SR + p] = part.vbar[i];
             } else {

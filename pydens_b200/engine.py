@@ -358,7 +358,7 @@ class FusedEngine:
 
     def _constraint_plan(self, num):
         """ Constraint `num` as one more launch of the same kernel family (reference :451-457): a plan whose
-        residual program is the traced constraint (no derivative channels), run on the constraint's own points
+        residual program is the traced constraint (on its own jet set or the equation's), run on the constraint's own points
         with 1/n weighting; its [grads | loss] buffer is then added to the step's.  None -> autograd adds it. """
         if num not in self._constraint_plans:
             entry = None
@@ -563,9 +563,16 @@ class FusedEngine:
         plan, or more terms / constraint points than the kernels take. """
         if 'equation' not in loss_terms:
             return None
-        entries = [self._constraint_plan(n) for n in self.solver._constraint_numbers(loss_terms)]
+        nums = self.solver._constraint_numbers(loss_terms)
+        entries = [self._constraint_plan(n) for n in nums]
         if any(e is None for e in entries) or len(entries) > _native.MAX_TERMS:
             return None
+        # the kernels run a term's program on the equation's jets: its plan carries no directions, or the same ones
+        eq = self.solver._traced
+        for n in nums:
+            tr = self.solver._lower_constraint(n)[0]
+            if tr.nf and (tr.order != 2 or eq.order != 2 or (tr.dirs, tr.dir_vecs, tr.ns) != (eq.dirs, eq.dir_vecs, eq.ns)):
+                return None
         if sum(e['n'] for e in entries) > _native.MAX_TERM_POINTS:
             return None
         if batch_size + sum(e['n'] for e in entries) > self.lib.pinn_multi_step_max_points(self.plan):

@@ -160,7 +160,9 @@ class Solver:
 
     def _lower_constraint(self, num):
         """ (traced constraint, its points as a [n, total] fp32 tensor) if constraint `num` can run as a fused
-        launch — one model evaluation at fixed points, combined pointwise — else None (autograd adds it). """
+        launch — one model evaluation at fixed points, differentiated along them or not, combined pointwise — else
+        None (autograd adds it).  A constraint with derivatives is traced in the equation's jet set where that carries
+        them (tracer.trace_constraint). """
         if num not in self._traced_constraints:
             lowered = None
             # a network of several outputs: its constraints are added by autograd (the constraint programs are scalar)
@@ -170,7 +172,7 @@ class Solver:
                     traced, args = tracer.trace_constraint(self.constraints[num], model.total,
                                                            initial_condition=model.raw_initial_condition,
                                                            ndims_spatial=model.ndims_spatial, run=self._tracing_run,
-                                                           criterion=self._crit_key)
+                                                           criterion=self._crit_key, layout=self._traced)
                     pts = self.reshape_and_concat(args).detach().to(torch.float32)
                     if pts.dim() != 2 or pts.shape[1] != model.total or pts.shape[0] < 1:
                         raise tracer.NotLowerable('constraint points do not have %d columns' % model.total)
@@ -293,7 +295,9 @@ class Solver:
         sampler     object with `.sample(size)`; None = U[0,1) on every column (reference :431).
                     Samplers from pydens_b200.sampler made of independent uniform / normal columns run
                     in-kernel; anything else is sampled on the host and copied per step.
-        loss_terms  'equation' and/or 'constraint_{k}' (reference :382-389).
+        loss_terms  'equation' and/or 'constraint_{k}' (reference :382-389).  A constraint that evaluates the model once
+                    at fixed points, optionally differentiated along them (`D(u(t0), t0)` with t0 requiring grad), and
+                    combines the result pointwise runs as a fused launch on its points; any other is added by autograd.
         optimizer   name from torch.optim; None re-uses the existing optimizer (reference :391-393).
         criterion   nn.MSELoss() (default), nn.L1Loss(), nn.HuberLoss(delta), nn.SmoothL1Loss(beta), mean or sum reduction,
                     train on the fused kernels (switching the criterion between fits rebuilds the engine); anything
@@ -303,7 +307,9 @@ class Solver:
                     launch of a persistent kernel.  Batches of at most 1024 points (the launch-bound regime of the
                     README example, batch_size=100, niters=1500) take this path by themselves, 50 steps per launch,
                     whenever the optimizer is plain Adam, there is one device, the equation is a loss term and every
-                    constraint term runs fused (at most 4 of them, 32 constraint points in all)
+                    constraint term runs fused (at most 4 of them, 32 constraint points in all) with no derivatives or
+                    only derivatives the equation's jet carries (u'(0) next to u'' + w^2 u = 0); a constraint that needs
+                    another derivative runs fused one launch per step, and so does the fit
                     (PYDENS_B200_AUTO_PERSISTENT=0 keeps one launch per step).
                     Decoupled weight decay (decoupled_weight_decay=True with weight_decay > 0, or optimizer='AdamW')
                     trains one step at a time with torch's Adam after the step kernel, and so does an optimizer state

@@ -828,9 +828,34 @@ def sym_D(y, x):
         raise NotLowerable('D() of a residual with several columns')
     if isinstance(y, Components):
         raise NotLowerable('D() of the whole output of a network with several outputs (select a component first)')
+    if _constraint_calls:                          # inside trace_constraint: x is a point tensor of the model call
+        return Sym(diff_coord(_as_expr(y), _constraint_column(x)))
     if not isinstance(x, Sym) or x.expr.kind != 'coord':
         raise NotLowerable('D(y, x): x must be one of the equation arguments')
     return Sym(diff_coord(_as_expr(y), x.expr.value))
+
+
+# the model calls of the constraint being traced (trace_constraint); a list rather than a ContextVar because the Solver
+# runs user callables in its own contextvars.Context
+_constraint_calls = []
+
+
+def _constraint_column(x):
+    """ The point column of the constraint's one model call that `x` was passed as (matched by identity): D(u(x0), x0)
+    is the derivative of u along that column. """
+    if isinstance(x, Sym):
+        raise NotLowerable('D with respect to the batch points inside a constraint')
+    calls = _constraint_calls[-1]
+    if not calls:
+        raise NotLowerable('D inside a constraint before it evaluates the model')
+    cols = [k for k, p in enumerate(calls[0]) if p is x]
+    if not cols:
+        raise NotLowerable('D(y, p) inside a constraint: p is not one of the tensors the model is evaluated at')
+    if len(cols) > 1:
+        raise NotLowerable('D(y, p) inside a constraint: p is passed as %d point columns' % len(cols))
+    if not isinstance(x, torch.Tensor) or not x.requires_grad:
+        raise NotLowerable('D(y, p) inside a constraint: p does not require grad')
+    return cols[0]
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1113,7 +1138,8 @@ def _leaves_of(exprs, kinds):
     return found
 
 
-def trace(equation, total, var_factory, initial_condition=None, ndims_spatial=0, run=None, criterion=None, n_out=1):
+def trace(equation, total, var_factory, initial_condition=None, ndims_spatial=0, run=None, criterion=None, n_out=1,
+          layout=None):
     """ Trace `equation(u, *xs)` (and `initial_condition(*x_spatial)` if callable).
 
     `var_factory(name)` is installed by the caller so that V(name, ...) returns `Sym(var(name))`
@@ -1123,6 +1149,8 @@ def trace(equation, total, var_factory, initial_condition=None, ndims_spatial=0,
     `n_out` = k in 2..4: the network has k outputs; the equation selects component j (Components), every component
     carries the same jet set, and the residual program follows the k-output convention of include/pinn_b200.h: slot
     j*C + c holds channel c of component j on entry, and dr/d(that channel) is left in slot eq_out[1] + j*C + c.
+    `layout`: a TracedEquation of order 2 whose jet set (dirs, dir_vecs, ns) is taken instead of the one the derivatives
+    call for — channels nothing uses get zero partials; raises NotLowerable if a derivative has no channel there.
     """
     run = run or (lambda f, *a: f(*a))
     xs = [Sym(coord(k)) for k in range(total)]
@@ -1137,35 +1165,45 @@ def trace(equation, total, var_factory, initial_condition=None, ndims_spatial=0,
     if any(len(mi) > 2 for mi in mis):
         if n_out > 1:
             raise NotLowerable('derivatives of order > 2 of a network with several outputs')
+        if layout is not None:
+            raise NotLowerable('derivatives of order > 2 in a second-order jet set')
         return _trace_high_order(T, rs, u_leaves, xs, total, initial_condition, ndims_spatial, run, criterion)
-    first, second, mixed = set(), set(), set()
-    for mi in mis:
-        if len(mi) == 1:
-            first.add(mi[0])
-        elif len(mi) == 2:
-            if mi[0] != mi[1]:
-                mixed.add(mi)                      # polarisation: u_ij = (u_vv - u_ii - u_jj) / 2, v = e_i + e_j
-                second.update(mi)
-            else:
-                second.add(mi[0])
-    first |= second
-    axes2, mixed, axes1 = sorted(second), sorted(mixed), sorted(first - second)
+    if layout is not None:
+        T.dirs, T.dir_vecs, T.ns = list(layout.dirs), [list(v) for v in layout.dir_vecs], layout.ns
+        nf, ns = len(T.dirs), T.ns
+        # the mixed directions e_i + e_j of the layout; D nests in either order, so both multi-indices map to it
+        mixed = [(d, tuple(k for k, v in enumerate(T.dir_vecs[d]) if v != 0.0)) for d in range(ns) if T.dirs[d] < 0]
+        mixed += [(d, (j, i)) for d, (i, j) in mixed]
+    else:
+        first, second, mixed = set(), set(), set()
+        for mi in mis:
+            if len(mi) == 1:
+                first.add(mi[0])
+            elif len(mi) == 2:
+                if mi[0] != mi[1]:
+                    mixed.add(mi)                      # polarisation: u_ij = (u_vv - u_ii - u_jj) / 2, v = e_i + e_j
+                    second.update(mi)
+                else:
+                    second.add(mi[0])
+        first |= second
+        axes2, mixed, axes1 = sorted(second), sorted(mixed), sorted(first - second)
 
-    def unit(k, *more):
-        return [1.0 if i in (k,) + more else 0.0 for i in range(total)]
-    T.dir_vecs = [unit(k) for k in axes2] + [unit(i, j) for i, j in mixed] + [unit(k) for k in axes1]
-    T.dirs = list(axes2) + [-1] * len(mixed) + list(axes1)
-    T.ns = len(axes2) + len(mixed)
-    nf, ns = len(T.dirs), T.ns
-    if nf > MAX_DIRS:
-        raise NotLowerable('more than %d derivative directions' % MAX_DIRS)
-    if n_out > 1 and nf > 4:
-        raise NotLowerable('more than 4 derivative directions in a network with several outputs')
-    if nf > 4:
-        # five / six directions (full Hessians in 3-D, Laplacians in 5-D / 6-D): the library holds ONE kernel per
-        # direction count there, the one in which every direction carries its second derivative — first-order-only
-        # directions are promoted (their second-order channel is computed and meets a zero adjoint seed)
-        T.ns = ns = nf
+        def unit(k, *more):
+            return [1.0 if i in (k,) + more else 0.0 for i in range(total)]
+        T.dir_vecs = [unit(k) for k in axes2] + [unit(i, j) for i, j in mixed] + [unit(k) for k in axes1]
+        T.dirs = list(axes2) + [-1] * len(mixed) + list(axes1)
+        T.ns = len(axes2) + len(mixed)
+        mixed = [(len(axes2) + n, ij) for n, ij in enumerate(mixed)]
+        nf, ns = len(T.dirs), T.ns
+        if nf > MAX_DIRS:
+            raise NotLowerable('more than %d derivative directions' % MAX_DIRS)
+        if n_out > 1 and nf > 4:
+            raise NotLowerable('more than 4 derivative directions in a network with several outputs')
+        if nf > 4:
+            # five / six directions (full Hessians in 3-D, Laplacians in 5-D / 6-D): the library holds ONE kernel per
+            # direction count there, the one in which every direction carries its second derivative — first-order-only
+            # directions are promoted (their second-order channel is computed and meets a zero adjoint seed)
+            T.ns = ns = nf
     C = 1 + nf + ns
     mapping = {}
     for q in range(n_out):                         # component q's jet: slots q*C .. q*C + C-1
@@ -1178,12 +1216,13 @@ def trace(equation, total, var_factory, initial_condition=None, ndims_spatial=0,
                 mapping[leaf((col,))] = chleaf(base + 1 + d)
                 if d < ns:
                     mapping[leaf((col, col))] = chleaf(base + 1 + nf + d)
-        for n, (i, j) in enumerate(mixed):
-            d = len(axes2) + n
+        for d, (i, j) in mixed:
             mapping[leaf((i, j))] = mul(const(0.5), sub(sub(chleaf(base + 1 + nf + d), mapping[leaf((i, i))]),
                                                         mapping[leaf((j, j))]))
     memo = {}
     rs = [substitute(r, mapping, memo) for r in rs]
+    if layout is not None and _leaves_of(rs, ('u',)):
+        raise NotLowerable('a derivative has no channel in the jet set')
     res = rs[0]
     chan = {}
     by_channel = {c: chleaf(c) for c in range(n_out * C)}
@@ -1344,14 +1383,30 @@ def _trace_high_order(T, rs, u_leaves, xs, total, initial_condition, ndims_spati
     return T
 
 
-def trace_constraint(constraint, total, initial_condition=None, ndims_spatial=0, run=None, criterion=None):
+def trace_constraint(constraint, total, initial_condition=None, ndims_spatial=0, run=None, criterion=None, layout=None):
     """ Trace a constraint `constraint(u, *xs)` (reference model_torch.py:451-457: `u` is a callable that
     evaluates the model at user points, the value is driven to zero by MSE) into the same program form as an
     equation.  Lowerable when the constraint evaluates the model ONCE, at concrete points, and combines that
     value pointwise with constants / variables: `lambda u, t: u(torch.tensor([0.5]))`, `… - 2.0`, `… ** 2`.
+    The value may be differentiated along a point tensor of that call, `D(u(t0), t0)` with t0 requiring grad: the
+    derivative along t0's column, nested as in an equation.
 
-    Returns (TracedEquation with no derivative directions, the tuple of point arguments of the one call).
+    A constraint without derivatives has no derivative directions (C = 1).  One with derivatives takes the jet set of
+    `layout` (the equation's TracedEquation) when that is of order 2 and carries every derivative it needs — the
+    persistent kernels run such a constraint next to the equation — else its own.
+
+    Returns (TracedEquation, the tuple of point arguments of the one call).
     """
+    traced, pts = _trace_constraint(constraint, total, initial_condition, ndims_spatial, run, criterion, None)
+    if traced.nf and layout is not None and layout.order == 2 and layout.n_out == 1:
+        try:
+            traced, pts = _trace_constraint(constraint, total, initial_condition, ndims_spatial, run, criterion, layout)
+        except NotLowerable:
+            pass
+    return traced, pts
+
+
+def _trace_constraint(constraint, total, initial_condition, ndims_spatial, run, criterion, layout):
     calls = []
 
     def u_at(*pts):
@@ -1362,12 +1417,14 @@ def trace_constraint(constraint, total, initial_condition=None, ndims_spatial=0,
         calls.append(pts)
         return Sym(uleaf())
 
-    traced = trace(lambda _u, *xs: constraint(u_at, *xs), total, None, initial_condition=initial_condition,
-                   ndims_spatial=ndims_spatial, run=run, criterion=criterion)
+    _constraint_calls.append(calls)
+    try:
+        traced = trace(lambda _u, *xs: constraint(u_at, *xs), total, None, initial_condition=initial_condition,
+                       ndims_spatial=ndims_spatial, run=run, criterion=criterion, layout=layout)
+    finally:
+        _constraint_calls.pop()
     if not calls:
         raise NotLowerable('constraint does not evaluate the model')
-    if traced.nf:
-        raise NotLowerable('derivatives inside a constraint')
     if leaves(traced.residual, ('coord',)):
         raise NotLowerable('constraint depends on the batch points')
     return traced, calls[0]
