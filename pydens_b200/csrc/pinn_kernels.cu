@@ -159,39 +159,48 @@ static bool wide_eligible(const pinn::DevPlan& h, int* max_width) {
     return true;
 }
 
+// The launch of pinn_step / pinn_step_allreduce / pinn_step_adam.
+struct StepLaunch {
+    StepKernelFn fn;
+    DevPlan plan;                            // the plan fn runs on: h, or its compact layout (build_remat_plan) under
+                                             // step_kernel_w12
+    int threads, smem, regs;
+    int points_per_cta;                      // per round: threads (thread kernels), Tile<KW>::T (tile kernels)
+    int tensor_core;                         // 0: a thread kernel; 1 / 2: the 64- / 128-wide tile kernel, whose grid
+                                             // PINN_WIDE_CTAS caps
+    bool state_in_smem;                      // the per-point state lives in shared memory, not in the spill area
+    size_t wacc_floats, spill_floats;        // workspace per CTA: gradient accumulators, spill area
+};
+
+// The launch of pinn_forward: a thread-forward kernel (FwdArgs) or the 128-wide tile kernel's forward-only form (StepArgs).
+struct ForwardLaunch {
+    void (*fn)(const DevPlan, const FwdArgs);
+    StepKernelFn tile_fn;
+    int threads, smem, points_per_cta, rows, row_scr;
+    size_t spill_floats;                     // workspace per CTA
+};
+
+// A persistent kernel (multi_step_kernel, or the tiny-batch cluster kernel) and its ensemble form; null where they do
+// not fit.  budget: the dynamic shared memory they can take (constraint programs with more slots).
+struct PersistentLaunch {
+    MultiKernelFn solo;
+    EnsembleKernelFn ensemble;
+    int threads, smem, budget;
+};
+
 struct PinnPlan {
     PinnSpec spec;
     DevPlan h;
     int device;
-    bool wide;                               // the tensor-core tile kernel runs the step
-    int wide_kw;                             // its width class: 64 or 128
-    StepKernelFn fn_wide;
-    MultiKernelFn fn_multi;                  // persistent multi-step kernel, or nullptr when it does not fit
-    int multi_threads, multi_smem;
-    MultiKernelFn fn_small;                  // tiny-batch (<= 128 points) variant, or nullptr
-    EnsembleKernelFn fn_multi_ens, fn_small_ens;   // their ensemble forms, or nullptr (same threads, any smem they take)
-    int small_smem;
-    int multi_budget, small_budget;          // dynamic shared memory the two can take (constraint programs with more slots)
-    int wide_ctas;                           // CTAs the tile kernel runs on (<= sm_count)
     const KernelSet* ks;                     // the kernels of this plan's jet set
-    StepKernelFn fn_smem, fn_gmem;           // the pair matching this plan (plain or general, or coupled_step_kernel);
-                                             // fn_smem is step_kernel_w12 when the twelve-warp form was placed
-    DevPlan hs;                              // the plan the thread step kernel runs on: h, or its compact layout
-                                             // (build_remat_plan) under step_kernel_w12
     bool coupled;                            // a network of 2..4 outputs: coupled_step_kernel / coupled_forward_kernel,
                                              // or the coupled form of the 128-wide tile kernel
     int sm_count;
     int smem_optin;
-    // step kernel launch config
-    bool gmem;
-    bool wacc_gmem;                          // the per-warp gradient accumulators live in the workspace, not in smem
-    int threads, smem_bytes, regs;
-    // forward kernel launch config
-    bool fwd_gmem;
-    bool fwd_wide;                           // pinn_forward runs the 128-wide tile kernel's forward-only form
-    int fwd_threads, fwd_smem_bytes, fwd_rows, fwd_row_scr;
+    StepLaunch step;
+    ForwardLaunch fwd;
+    PersistentLaunch multi, small;
 };
-
 
 extern "C" const char* pinn_last_error(void) { return g_err; }
 extern "C" int pinn_abi_version(void) { return PINN_ABI_VERSION; }
@@ -217,93 +226,104 @@ static int storage_floats(const DevPlan& h, int rows, int nw) {
     return rows * RS * nw > h.n_params ? rows * RS * nw : h.n_params;
 }
 
+// A kernel's attributes, and the dynamic shared memory it can take beside its static shared memory (64 B spare).
+static cudaError_t kernel_budget(const void* fn, int smem_optin, cudaFuncAttributes& fa, int& budget) {
+    const cudaError_t e = cudaFuncGetAttributes(&fa, fn);
+    if (e == cudaSuccess) budget = smem_optin - (int)fa.sharedSizeBytes - 64;
+    return e;
+}
+
+// Dynamic shared memory of a thread step kernel on `plan` at `nw` warps with `nwacc` gradient accumulators there (the
+// others live in the workspace); gmem: the per-point state lives in the spill area.
+static int step_smem_bytes(const DevPlan& plan, int nw, int nwacc, bool gmem) {
+    return smem_layout(plan.weights_floats, plan.n_params + 4, nwacc,
+                       gmem ? plan.n_params : storage_floats(plan, plan.rows_total, nw)).total_f * 4;
+}
+
+static StepLaunch thread_step(StepKernelFn fn, const DevPlan& plan, int regs, int nw, int nwacc, bool gmem) {
+    StepLaunch s = {};
+    s.fn = fn; s.plan = plan; s.regs = regs;
+    s.threads = s.points_per_cta = nw * 32;
+    s.smem = step_smem_bytes(plan, nw, nwacc, gmem);
+    s.state_in_smem = !gmem;
+    s.wacc_floats = nwacc ? 0 : (size_t)nw * (plan.n_params + 4);
+    s.spill_floats = gmem ? (size_t)nw * plan.rows_total * RS : 0;
+    return s;
+}
+
 // Thread kernel: per-point state in shared memory at the largest warp count that fits, or in the global spill area.
 // Every warp has a gradient accumulator of its own: in shared memory when it fits there too, else in the workspace.
-static int place_step_kernel(PinnPlan* p) {
+// fn_smem / fn_gmem: the pair matching this plan (plain or general, or coupled_step_kernel); fn_smem may be null.
+static int place_thread_step(const PinnPlan* p, StepKernelFn fn_smem, StepKernelFn fn_gmem, StepLaunch& s) {
     const DevPlan& h = p->h;
-    const int n_out_floats = h.n_params + 4;
-    const bool has_smem_form = p->fn_smem != nullptr;
     cudaFuncAttributes fa;
-    cudaError_t e = cudaFuncGetAttributes(&fa, (const void*)(has_smem_form ? p->fn_smem : p->fn_gmem));
+    int budget;
+    cudaError_t e = kernel_budget((const void*)(fn_smem ? fn_smem : fn_gmem), p->smem_optin, fa, budget);
     if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncGetAttributes: %s", cudaGetErrorString(e));
-    p->regs = fa.numRegs;
     const int max_nw = max_warps(fa, p->ks->maxt);
-    const int budget = p->smem_optin - (int)fa.sharedSizeBytes - 64;
     int best_nw = 0, best_nwacc = 0;                 // best_nwacc: accumulators in smem (best_nw), or 0 (workspace)
-    for (int nw = max_nw; nw >= 1 && !best_nw; --nw) {
-        for (int pass = 0; pass < 2 && !best_nw; ++pass) {
-            int nwacc = pass == 0 ? nw : 0;
-            SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, nwacc, storage_floats(h, h.rows_total, nw));
-            if (SL.total_f * 4 <= budget) { best_nw = nw; best_nwacc = nwacc; }
-        }
-    }
+    for (int nw = max_nw; nw >= 1 && !best_nw; --nw)
+        for (int nwacc : {nw, 0})
+            if (!best_nw && step_smem_bytes(h, nw, nwacc, false) <= budget) { best_nw = nw; best_nwacc = nwacc; }
     // PINN_FORCE_MODE=smem|gmem overrides the placement heuristic (experiments only)
     const char* force = getenv("PINN_FORCE_MODE");
+    const bool force_gmem = force && !strcmp(force, "gmem");
     bool use_smem = best_nw >= 4 || (best_nw >= 2 && max_nw <= 4);
     if (force && !strcmp(force, "smem") && best_nw >= 1) use_smem = true;
-    if (force && !strcmp(force, "gmem")) use_smem = false;
-    if (!has_smem_form) use_smem = false;
+    if (force_gmem || !fn_smem) use_smem = false;
     // three warps per scheduler: the twelve-warp form on the compact per-point layout, where its 384 threads fit (register
     // count, and the storage of twelve warps with their accumulators in shared memory or else in the workspace) and
     // outnumber the warps placed above (cfg2: 12 instead of 8)
     DevPlan hc;
     const StepKernelFn f12 = p->coupled ? nullptr : p->ks->step_w12;
-    if (f12 && !(force && !strcmp(force, "gmem")) && build_remat_plan(h, hc) && (!use_smem || best_nw < 12)) {
+    bool w12 = false;
+    if (f12 && !force_gmem && build_remat_plan(h, hc) && (!use_smem || best_nw < 12)) {
         cudaFuncAttributes f12a;
-        e = cudaFuncGetAttributes(&f12a, (const void*)f12);
+        int budget12;
+        e = kernel_budget((const void*)f12, p->smem_optin, f12a, budget12);
         if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncGetAttributes: %s", cudaGetErrorString(e));
-        const int budget12 = p->smem_optin - (int)f12a.sharedSizeBytes - 64;
-        for (int pass = 0; pass < 2 && max_warps(f12a, 384) == 12; ++pass) {
-            const int nwacc = pass == 0 ? 12 : 0;
-            const SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, nwacc, storage_floats(hc, hc.rows_total, 12));
-            if (SL.total_f * 4 > budget12) continue;
-            p->fn_smem = f12; p->hs = hc; p->regs = f12a.numRegs;
-            p->gmem = false; p->threads = 384; p->wacc_gmem = nwacc == 0; p->smem_bytes = SL.total_f * 4;
-            e = allow_max_smem((const void*)f12, p->smem_optin);
-            if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(smem=%d): %s", p->smem_bytes, cudaGetErrorString(e));
-            return PINN_OK;
-        }
+        for (int nwacc : {12, 0})
+            if (!w12 && max_warps(f12a, 384) == 12 && step_smem_bytes(hc, 12, nwacc, false) <= budget12) {
+                s = thread_step(f12, hc, f12a.numRegs, 12, nwacc, false);
+                w12 = true;
+            }
     }
-    if (use_smem) {
-        p->gmem = false; p->threads = best_nw * 32; p->wacc_gmem = best_nwacc == 0;
-        SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, best_nwacc, storage_floats(h, h.rows_total, best_nw));
-        p->smem_bytes = SL.total_f * 4;
-    } else {
+    if (!w12 && use_smem) {
+        s = thread_step(fn_smem, h, fa.numRegs, best_nw, best_nwacc, false);
+    } else if (!w12) {
         // activations spill to a global workspace; accumulators: in smem if they fit, else in the workspace too
-        e = cudaFuncGetAttributes(&fa, (const void*)p->fn_gmem);
+        e = cudaFuncGetAttributes(&fa, (const void*)fn_gmem);
         if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncGetAttributes: %s", cudaGetErrorString(e));
-        p->regs = fa.numRegs;
         int nw = max_warps(fa, p->ks->maxt);
         { const char* e2 = getenv("PINN_GMEM_WARPS"); if (e2 && atoi(e2) >= 1 && atoi(e2) <= nw) nw = atoi(e2); }   // experiments
-        int nwacc = nw;
-        SmemLayout SL = smem_layout(h.weights_floats, n_out_floats, nwacc, h.n_params);
-        if (SL.total_f * 4 > budget) { nwacc = 0; SL = smem_layout(h.weights_floats, n_out_floats, 0, h.n_params); }
-        if (SL.total_f * 4 > budget) return fail(PINN_E_UNSUPPORTED, "network too large: %d B of weights do not fit shared memory", SL.total_f * 4);
-        p->gmem = true; p->threads = nw * 32; p->wacc_gmem = nwacc == 0; p->smem_bytes = SL.total_f * 4;
+        const int nwacc = step_smem_bytes(h, nw, nw, true) <= budget ? nw : 0;
+        if (step_smem_bytes(h, nw, nwacc, true) > budget)
+            return fail(PINN_E_UNSUPPORTED, "network too large: %d B of weights do not fit shared memory", step_smem_bytes(h, nw, 0, true));
+        s = thread_step(fn_gmem, h, fa.numRegs, nw, nwacc, true);
     }
-    e = allow_max_smem((const void*)(p->gmem ? p->fn_gmem : p->fn_smem), p->smem_optin);
-    if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(smem=%d): %s", p->smem_bytes, cudaGetErrorString(e));
+    e = allow_max_smem((const void*)s.fn, p->smem_optin);
+    if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(smem=%d): %s", s.smem, cudaGetErrorString(e));
     return PINN_OK;
 }
 
-// Forward kernel: eight warps, per-point state in shared memory when it fits, else in the global spill area.
-static int place_forward_kernel(PinnPlan* p) {
+// Forward kernel: eight warps, per-point state (`rows` rows) in shared memory when it fits, else in the global spill area.
+static int place_forward_kernel(const PinnPlan* p, int rows, int row_scr, ForwardLaunch& f) {
     const DevPlan& h = p->h;
     const int nw = 8;
-    SmemLayout SL = smem_layout(h.weights_floats, 0, 0, storage_floats(h, p->fwd_rows, nw));
-    if (SL.total_f * 4 <= p->smem_optin - 64) { p->fwd_gmem = false; }
-    else { p->fwd_gmem = true; SL = smem_layout(h.weights_floats, 0, 0, h.n_params); }
-    p->fwd_threads = nw * 32; p->fwd_smem_bytes = SL.total_f * 4;
-    if (p->fwd_smem_bytes > p->smem_optin - 64) return fail(PINN_E_UNSUPPORTED, "network too large for shared memory");
-    const void* fn = p->coupled ? (p->fwd_gmem ? (const void*)coupled_forward_kernel<true> : (const void*)coupled_forward_kernel<false>)
-                                : (p->fwd_gmem ? (const void*)forward_kernel<true> : (const void*)forward_kernel<false>);
-    const cudaError_t e = allow_max_smem(fn, p->smem_optin);
+    int smem = smem_layout(h.weights_floats, 0, 0, storage_floats(h, rows, nw)).total_f * 4;
+    const bool gmem = smem > p->smem_optin - 64;
+    if (gmem) smem = smem_layout(h.weights_floats, 0, 0, h.n_params).total_f * 4;
+    if (smem > p->smem_optin - 64) return fail(PINN_E_UNSUPPORTED, "network too large for shared memory");
+    f = {};
+    f.fn = p->coupled ? (gmem ? coupled_forward_kernel<true> : coupled_forward_kernel<false>)
+                      : (gmem ? forward_kernel<true> : forward_kernel<false>);
+    f.threads = f.points_per_cta = nw * 32; f.smem = smem; f.rows = rows; f.row_scr = row_scr;
+    f.spill_floats = gmem ? (size_t)nw * rows * RS : 0;
+    const cudaError_t e = allow_max_smem((const void*)f.fn, p->smem_optin);
     if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(fwd): %s", cudaGetErrorString(e));
     return PINN_OK;
 }
 
-// Persistent multi-step kernel (small batches): per-point state + parameters + Adam moments in shared memory.  Left
-// out when the jet set has none or the network does not fit.
 // Dynamic shared memory of multi_step_kernel at `nw` warps and `rows` per-point rows.
 static int multi_smem_bytes(const DevPlan& h, int nw, int rows) {
     const int n_out_floats = h.n_params + 4;
@@ -311,58 +331,32 @@ static int multi_smem_bytes(const DevPlan& h, int nw, int rows) {
     return (smem_layout(h.weights_floats, n_out_floats, nw, storage_floats(h, rows, nw)).total_f + extra) * 4;
 }
 
-static void place_multi_kernel(PinnPlan* p) {
-    p->fn_multi = nullptr; p->multi_threads = 0; p->multi_smem = 0; p->multi_budget = 0; p->fn_multi_ens = nullptr;
-    const MultiKernelFn f = p->ks->multi;
-    if (!f) return;
-    cudaFuncAttributes fm;
-    if (cudaFuncGetAttributes(&fm, (const void*)f) == cudaSuccess) {
-        const DevPlan& h = p->h;
-        const int mbudget = p->smem_optin - (int)fm.sharedSizeBytes - 64;
-        for (int nw = max_warps(fm, p->ks->maxt); nw >= 1 && !p->fn_multi; --nw) {
-            const int bytes = multi_smem_bytes(h, nw, h.rows_total);
-            if (bytes <= mbudget) {
-                p->fn_multi = f; p->multi_threads = nw * 32;
-                p->multi_smem = bytes; p->multi_budget = mbudget;
-            }
+// A persistent kernel `f` (compiled for maxt threads) at the most warps whose dynamic shared memory, bytes(nw), fits, and
+// its ensemble form `fe` where that runs as many threads in at least as much shared memory.  Null where the jet set has
+// none or they do not fit.
+template <class Bytes>
+static PersistentLaunch place_persistent(const PinnPlan* p, MultiKernelFn f, EnsembleKernelFn fe, int maxt, Bytes bytes) {
+    PersistentLaunch k = {};
+    cudaFuncAttributes fa;
+    int budget;
+    if (f && kernel_budget((const void*)f, p->smem_optin, fa, budget) == cudaSuccess)
+        for (int nw = max_warps(fa, maxt); nw >= 1; --nw) {
+            if (bytes(nw) > budget) continue;
+            if (allow_max_smem((const void*)f, p->smem_optin) == cudaSuccess) k = {f, nullptr, nw * 32, bytes(nw), budget};
+            break;
         }
-        if (p->fn_multi && allow_max_smem((const void*)f, p->smem_optin) != cudaSuccess) p->fn_multi = nullptr;
-    }
-    p->fn_multi_ens = nullptr;
-    const EnsembleKernelFn fe = p->ks->multi_ensemble;
-    if (p->fn_multi && fe && cudaFuncGetAttributes(&fm, (const void*)fe) == cudaSuccess &&
-        max_warps(fm, p->ks->maxt) * 32 >= p->multi_threads && p->smem_optin - (int)fm.sharedSizeBytes - 64 >= p->multi_budget &&
-        allow_max_smem((const void*)fe, p->smem_optin) == cudaSuccess)
-        p->fn_multi_ens = fe;
+    if (k.solo && fe && kernel_budget((const void*)fe, p->smem_optin, fa, budget) == cudaSuccess &&
+        max_warps(fa, k.threads) * 32 >= k.threads && budget >= k.budget && allow_max_smem((const void*)fe, p->smem_optin) == cudaSuccess)
+        k.ensemble = fe;
     (void)cudaGetLastError();
-}
-
-// Tiny batches: the (point, unit)-parallel loop kernel, for plain dense chains whose jets fit shared memory.  Left out
-// when the jet set has none (more than four directions, orders 3 / 4).
-static void place_small_kernel(PinnPlan* p) {
-    p->fn_small = nullptr; p->small_smem = 0; p->small_budget = 0; p->fn_small_ens = nullptr;
-    const MultiKernelFn f = p->ks->small;
-    if (!f) return;
-    const DevPlan& h = p->h;
-    for (int l = 0; l < h.n_layers; ++l) if (h.layer[l].skip_src >= 0 || h.layer[l].post_base >= 0) return;
-    const int bytes = small::make_layout(h).total * 4;
-    cudaFuncAttributes fs;
-    if (cudaFuncGetAttributes(&fs, (const void*)f) == cudaSuccess && bytes <= p->smem_optin - (int)fs.sharedSizeBytes - 64 &&
-        allow_max_smem((const void*)f, p->smem_optin) == cudaSuccess) {
-        p->fn_small = f; p->small_smem = bytes; p->small_budget = p->smem_optin - (int)fs.sharedSizeBytes - 64;
-        const EnsembleKernelFn fe = p->ks->small_ensemble;
-        if (fe && cudaFuncGetAttributes(&fs, (const void*)fe) == cudaSuccess &&
-            p->smem_optin - (int)fs.sharedSizeBytes - 64 >= p->small_budget && allow_max_smem((const void*)fe, p->smem_optin) == cudaSuccess)
-            p->fn_small_ens = fe;
-    }
-    (void)cudaGetLastError();
+    return k;
 }
 
 // Wide networks: the tensor-core tile kernel takes the step (PINN_FORCE_KERNEL=thread|wide|wide128 overrides).
 // thread_rc is how the thread kernel's placement (step and forward) went: a network whose weights do not fit its
 // shared memory goes to the 128-wide class when that class covers it; otherwise that failure is the plan's.
-static int place_wide_kernel(PinnPlan* p, int order, int thread_rc) {
-    p->wide = false; p->fn_wide = nullptr; p->wide_ctas = p->sm_count; p->wide_kw = 64; p->fwd_wide = false;
+// Fills `s` where the tile kernel takes the step; returns thread_rc where it does not.
+static int place_tile_step(const PinnPlan* p, int order, int thread_rc, StepLaunch& s) {
     int mw = 0;
     const char* fk = getenv("PINN_FORCE_KERNEL");
     const bool eligible = order < 3 && wide_eligible(p->h, &mw);
@@ -395,15 +389,23 @@ static int place_wide_kernel(PinnPlan* p, int order, int thread_rc) {
     cudaFuncAttributes fa;
     e = cudaFuncGetAttributes(&fa, (const void*)f);
     if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncGetAttributes(wide): %s", cudaGetErrorString(e));
-    p->fn_wide = f;
-    p->wide = true; p->wide_kw = kw; p->gmem = true; p->threads = wide::NT; p->wacc_gmem = false; p->hs = p->h;
-    p->smem_bytes = smem; p->regs = fa.numRegs;
-    if (thread_rc != PINN_OK) {                 // the forward kernel does not hold this network either
-        const void* ff = p->coupled ? (const void*)wide::wide128_coupled_forward_kernel : (const void*)wide::wide128_forward_kernel;
-        e = cudaFuncSetAttribute(ff, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(wide forward, smem=%d): %s", smem, cudaGetErrorString(e));
-        p->fwd_wide = true; p->fwd_gmem = false;
-    }
+    s = {};
+    s.fn = f; s.plan = p->h; s.threads = wide::NT; s.smem = smem; s.regs = fa.numRegs;
+    s.points_per_cta = kw == 128 ? wide::Tile<128>::T : wide::Tile<64>::T;
+    s.tensor_core = kw == 128 ? 2 : 1;
+    s.wacc_floats = kw == 128 ? wide::Tile<128>::WACC_FLOATS : 0;
+    s.spill_floats = wide::spill_floats_per_cta(p->h.n_layers, 1 + p->h.nf + p->h.ns);
+    return PINN_OK;
+}
+
+// The 128-wide tile kernel's forward-only form, for the networks the thread-forward kernel does not hold.
+static int place_tile_forward(const PinnPlan* p, ForwardLaunch& f) {
+    const StepKernelFn ff = p->coupled ? wide::wide128_coupled_forward_kernel : wide::wide128_forward_kernel;
+    const int smem = p->coupled ? wide::Tile<128, true>::SMEM_BYTES : wide::Tile<128>::SMEM_BYTES;
+    const cudaError_t e = cudaFuncSetAttribute((const void*)ff, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaFuncSetAttribute(wide forward, smem=%d): %s", smem, cudaGetErrorString(e));
+    f = {};
+    f.tile_fn = ff; f.threads = wide::NT; f.smem = smem; f.points_per_cta = wide::Tile<128>::T;
     return PINN_OK;
 }
 
@@ -411,9 +413,10 @@ extern "C" int pinn_plan_create(const PinnSpec* s, int device, PinnPlan** out) {
     if (!s || !out) return fail(PINN_E_INVALID, "null argument");
     std::unique_ptr<PinnPlan> p(new (std::nothrow) PinnPlan());
     if (!p) return fail(PINN_E_INVALID, "out of memory");
+    int fwd_rows, fwd_row_scr;
     {
         char msg[256];
-        const int rc = build_dev_plan(s, p->h, p->fwd_rows, p->fwd_row_scr, msg, sizeof(msg), 4);
+        const int rc = build_dev_plan(s, p->h, fwd_rows, fwd_row_scr, msg, sizeof(msg), 4);
         if (rc) return fail(rc, "%s", msg);
     }
     // orders 3 / 4 take whole jets per direction (pinn_hi_kernel.cuh), one kernel per (nf, order); their plans have ns = 0
@@ -426,18 +429,17 @@ extern "C" int pinn_plan_create(const PinnSpec* s, int device, PinnPlan** out) {
                     s->nf > 4 ? " (more than 4 derivative directions: every direction must carry its second derivative, ns = nf)" : "");
     // a set with the general global-memory form only serves plain plans with it
     const int gen = p->h.general ? 1 : 0;
-    p->fn_smem = p->ks->step[gen][0];
-    p->fn_gmem = p->ks->step[gen][1] ? p->ks->step[gen][1] : p->ks->step[1][1];
+    StepKernelFn fn_smem = p->ks->step[gen][0];
+    StepKernelFn fn_gmem = p->ks->step[gen][1] ? p->ks->step[gen][1] : p->ks->step[1][1];
     // networks of 2..4 outputs: their own step kernels (build_dev_plan has refused what those do not cover)
     p->coupled = p->h.layer[p->h.n_layers - 1].n_out > 1;
     if (p->coupled) {
         if (!p->ks->coupled[1]) return fail(PINN_E_UNSUPPORTED, "no kernel for a network of several outputs with nf=%d ns=%d", p->h.nf, p->h.ns);
-        p->fn_smem = p->ks->coupled[0];
-        p->fn_gmem = p->ks->coupled[1];
+        fn_smem = p->ks->coupled[0];
+        fn_gmem = p->ks->coupled[1];
     }
     p->spec = *s;
     p->device = device;
-    p->hs = p->h;
 
     cudaError_t e = cudaSetDevice(device);
     if (e != cudaSuccess) return fail(PINN_E_CUDA, "cudaSetDevice(%d): %s", device, cudaGetErrorString(e));
@@ -449,15 +451,27 @@ extern "C" int pinn_plan_create(const PinnSpec* s, int device, PinnPlan** out) {
     p->smem_optin = (int)prop.sharedMemPerBlockOptin;
 
     // the thread kernels (step and forward); a network whose weights do not fit their shared memory can still go to
-    // the 128-wide tile kernel, which stages one layer at a time (place_wide_kernel)
-    int thread_rc = place_step_kernel(p.get());
-    if (thread_rc == PINN_OK) thread_rc = place_forward_kernel(p.get());
+    // the 128-wide tile kernel, which stages one layer at a time (place_tile_step)
+    StepLaunch thread = {}, tile = {};
+    int thread_rc = place_thread_step(p.get(), fn_smem, fn_gmem, thread);
+    if (thread_rc == PINN_OK) thread_rc = place_forward_kernel(p.get(), fwd_rows, fwd_row_scr, p->fwd);
     if (thread_rc != PINN_OK && thread_rc != PINN_E_UNSUPPORTED) return thread_rc;
     if (!p->coupled) {                           // the persistent multi-step kernels take networks of one output only
-        place_multi_kernel(p.get());
-        place_small_kernel(p.get());
+        // multi_step_kernel (small batches): per-point state + parameters + Adam moments in shared memory
+        const DevPlan& h = p->h;
+        p->multi = place_persistent(p.get(), p->ks->multi, p->ks->multi_ensemble, p->ks->maxt,
+                                    [&](int nw) { return multi_smem_bytes(h, nw, h.rows_total); });
+        // tiny batches: the (point, unit)-parallel cluster kernel, for plain dense chains whose jets fit shared memory
+        bool chain = true;
+        for (int l = 0; l < h.n_layers; ++l) chain = chain && h.layer[l].skip_src < 0 && h.layer[l].post_base < 0;
+        if (chain)
+            p->small = place_persistent(p.get(), p->ks->small, p->ks->small_ensemble, small::NT,
+                                        [&](int) { return small::make_layout(h).total * 4; });
     }
-    if (int rc = place_wide_kernel(p.get(), order, thread_rc)) return rc;
+    if (int rc = place_tile_step(p.get(), order, thread_rc, tile)) return rc;
+    p->step = tile.fn ? tile : thread;
+    if (tile.fn && thread_rc != PINN_OK)          // the forward kernel does not hold this network either
+        if (int rc = place_tile_forward(p.get(), p->fwd)) return rc;
     *out = p.release();
     return PINN_OK;
 }
@@ -468,43 +482,27 @@ extern "C" int pinn_plan_destroy(PinnPlan* p) {
     return PINN_OK;
 }
 
-static int grid_for(const PinnPlan* p, long long n_points, int threads) {
-    long long tiles = (n_points + 31) / 32;
-    long long ctas = (tiles + threads / 32 - 1) / (threads / 32);
-    if (ctas > p->sm_count) ctas = p->sm_count;
-    if (ctas < 1) ctas = 1;
-    return (int)ctas;
+// CTAs of a launch over n points at `per_cta` points per CTA and round, at most `cap`.
+static int ctas(long long n_points, int per_cta, int cap) {
+    const long long c = (n_points + per_cta - 1) / per_cta;
+    return (int)(c < cap ? c : cap);
 }
 
 // workspace layout: [ticket: 256 B][partials: sm_count x n_out_floats][accumulators][spill]; the accumulators are the
 // thread kernel's per-warp gradient accumulators (sm_count x warps x n_out_floats) when they do not fit shared memory,
-// or the 128-wide tile kernel's hidden->hidden weight gradients (sm_count x 4 x 128 x 128, 256 KB per CTA)
-static size_t ws_partials_off() { return 256; }
-static size_t ws_wacc_off(const PinnPlan* p) {
-    size_t b = ws_partials_off() + (size_t)p->sm_count * (p->h.n_params + 4) * sizeof(float);
-    return (b + 255) & ~(size_t)255;
-}
-static size_t ws_wacc_bytes(const PinnPlan* p) {
-    if (p->wide) return p->wide_kw == 128 ? (size_t)p->sm_count * wide::Tile<128>::WACC_FLOATS * sizeof(float) : 0;
-    return p->wacc_gmem ? (size_t)p->sm_count * (p->threads / 32) * (p->h.n_params + 4) * sizeof(float) : 0;
-}
+// or the 128-wide tile kernel's hidden->hidden weight gradients (sm_count x 4 x 128 x 128, 256 KB per CTA); the spill
+// area is shared by the step and forward launches.
+static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+static size_t ws_wacc_off(const PinnPlan* p) { return align256(256 + (size_t)p->sm_count * (p->h.n_params + 4) * sizeof(float)); }
 static size_t ws_spill_off(const PinnPlan* p) {
-    size_t b = ws_wacc_off(p) + ws_wacc_bytes(p);
-    return (b + 255) & ~(size_t)255;
+    return align256(ws_wacc_off(p) + (size_t)p->sm_count * p->step.wacc_floats * sizeof(float));
 }
 
 extern "C" size_t pinn_workspace_bytes(const PinnPlan* p, int64_t n_points) {
     if (!p) return 0;
-    size_t b = ws_spill_off(p);
-    size_t spill = 0;
-    if (p->wide) spill = (size_t)p->sm_count * pinn::wide::spill_floats_per_cta(p->h.n_layers, 1 + p->h.nf + p->h.ns) * sizeof(float);
-    else if (p->gmem) spill = (size_t)p->sm_count * (p->threads / 32) * p->h.rows_total * RS * sizeof(float);
-    if (p->fwd_gmem) {
-        size_t f = (size_t)p->sm_count * (p->fwd_threads / 32) * p->fwd_rows * RS * sizeof(float);
-        if (f > spill) spill = f;
-    }
     (void)n_points;
-    return b + spill;
+    const size_t spill = p->step.spill_floats > p->fwd.spill_floats ? p->step.spill_floats : p->fwd.spill_floats;
+    return ws_spill_off(p) + (size_t)p->sm_count * spill * sizeof(float);
 }
 
 extern "C" int pinn_out_floats(const PinnPlan* p) { return p ? p->h.n_params + 4 : 0; }
@@ -723,17 +721,18 @@ static int step_impl(const PinnPlan* cp, const PinnComm* comm, const float* para
     if (comm && (!comm->connected || comm->bytes != comm_bytes(p->h.n_params + 4, comm->world)))
         return fail(PINN_E_INVALID, "communicator is not connected or belongs to another plan");
     cudaStream_t st = (cudaStream_t)stream;
-    DevPlan plan = p->hs;
+    const StepLaunch& s = p->step;
+    DevPlan plan = s.plan;
     if (!points) { int rc = resolve_cols(p, cols, plan.cols); if (rc) return rc; }
     StepArgs a;
     a.params = params; a.points = points; a.seed = seed;
     a.step_ptr = step_counter; a.step_val = step_value; a.point_offset = point_offset;
     a.n_points = n_points; a.inv_n = inv_global_n; a.out = grads_and_loss; a.residual = residual_out;
     a.ticket = reinterpret_cast<unsigned int*>(workspace);
-    a.partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_partials_off());
+    a.partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
     a.spill = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_spill_off(p));
-    a.wacc = ws_wacc_bytes(p) ? reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_wacc_off(p)) : nullptr;
-    a.rows_total = p->hs.rows_total;
+    a.wacc = s.wacc_floats ? reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_wacc_off(p)) : nullptr;
+    a.rows_total = s.plan.rows_total;
     a.adam_m = nullptr; a.adam_v = nullptr; a.adam_mask = nullptr; a.adam_steps = nullptr; a.adam_n_steps = 0;
     a.adam_lr = a.adam_beta1 = a.adam_beta2 = a.adam_eps = a.adam_wd = 0.0f;
     a.ring = nullptr; a.ring_len = 1;
@@ -759,17 +758,9 @@ static int step_impl(const PinnPlan* cp, const PinnComm* comm, const float* para
     a.comm_rank = comm ? comm->rank : 0;
     a.comm_world = comm ? comm->world : 0;
     for (int r = 0; r < PINN_COMM_MAX_RANKS; ++r) a.comm_peers[r] = comm ? comm->peers[r] : nullptr;
-    if (p->wide) {
-        const int T = p->wide_kw == 128 ? wide::Tile<128>::T : wide::Tile<64>::T;
-        long long tiles = (n_points + T - 1) / T;
-        int max_ctas = p->wide_ctas;
-        { const char* e = getenv("PINN_WIDE_CTAS"); if (e && atoi(e) >= 1 && atoi(e) <= p->sm_count) max_ctas = atoi(e); }   // experiments
-        const int grid = (int)(tiles < max_ctas ? tiles : max_ctas);
-        return launch_step(p->fn_wide, grid, p->threads, p->smem_bytes, st, plan, a);
-    }
-    const int grid = grid_for(p, n_points, p->threads);
-    StepKernelFn fn = p->gmem ? p->fn_gmem : p->fn_smem;
-    return launch_step(fn, grid, p->threads, p->smem_bytes, st, plan, a);
+    int cap = p->sm_count;
+    if (s.tensor_core) { const char* e = getenv("PINN_WIDE_CTAS"); if (e && atoi(e) >= 1 && atoi(e) <= p->sm_count) cap = atoi(e); }   // experiments
+    return launch_step(s.fn, ctas(n_points, s.points_per_cta, cap), s.threads, s.smem, st, plan, a);
 }
 
 extern "C" int pinn_step(const PinnPlan* plan, const float* params, const float* points, const PinnColumn* cols,
@@ -801,7 +792,7 @@ extern "C" int pinn_step_adam(const PinnPlan* plan, const PinnComm* comm, float*
 
 extern "C" int pinn_multi_step_max_points(const PinnPlan* p) {
     // one CTA walks the batch tile by tile: any batch works, but the kernel is meant for the launch-bound regime
-    return (p && p->fn_multi) ? 4096 : ((p && p->fn_small) ? 8 * pinn::small::BP : 0);
+    return (p && p->multi.solo) ? 4096 : ((p && p->small.solo) ? 8 * pinn::small::BP : 0);
 }
 
 // A constraint term's plan next to the plan it trains with (build_dev_term).
@@ -812,18 +803,19 @@ static int term_matches(const PinnPlan* p, const PinnPlan* q, DevTerm& t) {
 }
 
 // What pinn_multi_step_terms and pinn_multi_step_ensemble share: the checks of the shared arguments and the terms, the
-// by-value plan and arguments, and the kernel the columns go to — the cluster kernel at nc CTAs, or the multi-step kernel.
+// by-value plan and arguments, and the kernel the columns go to — the cluster kernel at nc CTAs per member, or the
+// multi-step kernel at one CTA per member (nc = 0).
 struct MultiLaunch {
     DevPlan plan;
     MultiArgs a;
-    bool small;
+    const PersistentLaunch* k;
     int nc, smem;
 };
 
 static int multi_setup(PinnPlan* p, int64_t n_points, int k_steps, float lr, float beta1, float beta2, float eps,
                        float weight_decay, int64_t ring_len, float point_weight, int n_terms, const PinnTerm* terms,
                        MultiLaunch& L) {
-    if (!p->fn_multi && !p->fn_small) return fail(PINN_E_UNSUPPORTED, "the persistent multi-step kernels do not fit this network in shared memory");
+    if (!p->multi.solo && !p->small.solo) return fail(PINN_E_UNSUPPORTED, "the persistent multi-step kernels do not fit this network in shared memory");
     if (n_terms < 0 || n_terms > PINN_MAX_TERMS || (n_terms > 0 && !terms))
         return fail(PINN_E_INVALID, "pinn_multi_step_terms: %d terms (0..%d)", n_terms, PINN_MAX_TERMS);
     if (!(point_weight >= 0.0f) || point_weight > 3.0e38f) return fail(PINN_E_INVALID, "point_weight must be finite and >= 0");
@@ -860,11 +852,14 @@ static int multi_setup(PinnPlan* p, int64_t n_points, int k_steps, float lr, flo
     a.rows_total = rows;
     // batches of at most 128 points: the (point, unit)-parallel kernel (PINN_MULTI_KERNEL=tile forces the other one)
     const char* mk = getenv("PINN_MULTI_KERNEL");
-    L.small = p->fn_small && n_cols <= 8 * pinn::small::BP && (n_cols <= 256 || !p->fn_multi) &&
-              !(mk && !strcmp(mk, "tile") && p->fn_multi);
-    if (L.small) {
-        L.smem = n_slots == p->h.n_slots ? p->small_smem : small::make_layout(L.plan).total * 4;
-        if (L.smem > p->small_budget) return fail(PINN_E_UNSUPPORTED, "the constraint programs' scratch slots do not fit shared memory");
+    const bool small = p->small.solo && n_cols <= 8 * pinn::small::BP && (n_cols <= 256 || !p->multi.solo) &&
+                       !(mk && !strcmp(mk, "tile") && p->multi.solo);
+    L.k = small ? &p->small : &p->multi;
+    if (small) L.smem = n_slots == p->h.n_slots ? L.k->smem : small::make_layout(L.plan).total * 4;
+    else       L.smem = rows == p->h.rows_total ? L.k->smem : multi_smem_bytes(p->h, L.k->threads / 32, rows);
+    if (L.smem > L.k->budget) return fail(PINN_E_UNSUPPORTED, "the constraint programs' scratch slots do not fit shared memory");
+    L.nc = 0;
+    if (small) {
         // a cluster of up to 8 CTAs (8 SMs) shares the columns, ~16 per CTA at least; PINN_SMALL_CLUSTER overrides
         int nc = (int)((n_cols + 15) / 16);
         if (nc > 8) nc = 8;
@@ -872,21 +867,23 @@ static int multi_setup(PinnPlan* p, int64_t n_points, int k_steps, float lr, flo
         while ((n_cols + nc - 1) / nc > pinn::small::BP) ++nc;
         if (nc == 3) nc = 4; else if (nc > 4 && nc < 8) nc = 8;         // cluster sizes 1, 2, 4, 8
         L.nc = nc;
-    } else {
-        L.nc = 1;
-        L.smem = rows == p->h.rows_total ? p->multi_smem : multi_smem_bytes(p->h, p->multi_threads / 32, rows);
-        if (L.smem > p->multi_budget) return fail(PINN_E_UNSUPPORTED, "the constraint programs' scratch slots do not fit shared memory");
     }
     return PINN_OK;
 }
 
-// The cluster kernel on n_members clusters of L.nc CTAs (member c: CTAs c * nc .. c * nc + nc - 1).
+// The persistent kernel of L for n_members members: the multi-step kernel on one CTA each, or the cluster kernel on
+// n_members clusters of L.nc CTAs (member c: CTAs c * nc .. c * nc + nc - 1).
 template <class... Args>
-static int launch_clusters(void (*fn)(const DevPlan, const MultiArgs, Args...), const MultiLaunch& L, int n_members,
-                           void* stream, const Args&... extra) {
+static int launch_persistent(void (*fn)(const DevPlan, const MultiArgs, Args...), const MultiLaunch& L, int n_members,
+                             void* stream, const Args&... extra) {
+    if (!L.nc) {
+        fn<<<n_members, L.k->threads, L.smem, (cudaStream_t)stream>>>(L.plan, L.a, extra...);
+        CUDA_TRY(cudaGetLastError());
+        return PINN_OK;
+    }
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(L.nc * n_members); cfg.blockDim = dim3(pinn::small::NT); cfg.dynamicSmemBytes = L.smem;
+    cfg.gridDim = dim3(L.nc * n_members); cfg.blockDim = dim3(L.k->threads); cfg.dynamicSmemBytes = L.smem;
     cfg.stream = (cudaStream_t)stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -918,10 +915,7 @@ extern "C" int pinn_multi_step_terms(const PinnPlan* cp, float* params, float* e
     a.step_counter = reinterpret_cast<unsigned long long*>(step_counter);
     a.opt_step0 = opt_step0;
     a.losses_ring = losses_ring;
-    if (L.small) return launch_clusters(p->fn_small, L, 1, stream);
-    p->fn_multi<<<1, p->multi_threads, L.smem, (cudaStream_t)stream>>>(L.plan, a);
-    CUDA_TRY(cudaGetLastError());
-    return PINN_OK;
+    return launch_persistent(L.k->solo, L, 1, stream);
 }
 
 extern "C" int pinn_multi_step_ensemble(const PinnPlan* cp, int n_members, const PinnMember* members, int64_t n_points,
@@ -945,15 +939,12 @@ extern "C" int pinn_multi_step_ensemble(const PinnPlan* cp, int n_members, const
     static thread_local DevMembers table;                            // 10 KB
     if (int rc = multi_setup(p, n_points, k_steps, lr, beta1, beta2, eps, weight_decay, ring_len, point_weight, n_terms, terms, L))
         return rc;
-    if (L.small ? !p->fn_small_ens : !p->fn_multi_ens)
+    if (!L.k->ensemble)
         return fail(PINN_E_UNSUPPORTED, "the ensemble form of the persistent kernel does not fit this network");
     if (sample) { int rc = resolve_cols(p, cols, L.plan.cols); if (rc) return rc; }
     memset(&table, 0, sizeof(table));
     memcpy(table.m, members, sizeof(PinnMember) * (size_t)n_members);
-    if (L.small) return launch_clusters(p->fn_small_ens, L, n_members, stream, table);
-    p->fn_multi_ens<<<n_members, p->multi_threads, L.smem, (cudaStream_t)stream>>>(L.plan, L.a, table);
-    CUDA_TRY(cudaGetLastError());
-    return PINN_OK;
+    return launch_persistent(L.k->ensemble, L, n_members, stream, table);
 }
 
 extern "C" int pinn_multi_step(const PinnPlan* p, float* params, float* exp_avg, float* exp_avg_sq, const float* mask,
@@ -974,28 +965,19 @@ extern "C" int pinn_forward(const PinnPlan* p, const float* params, const float*
     if (((uintptr_t)points) & 3u) return fail(PINN_E_ALIGN, "points must be 4-byte aligned");
     if (workspace_bytes < pinn_workspace_bytes(p, n_points)) return fail(PINN_E_WORKSPACE, "workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
-    if (p->fwd_wide) {                         // u of every point goes to `out` of the step arguments
+    const ForwardLaunch& f = p->fwd;
+    const int grid = ctas(n_points, f.points_per_cta, p->sm_count);
+    if (f.tile_fn) {                           // u of every point (coupled: u_out [n, k]) goes to `out` of the step arguments
         StepArgs w;
         memset(&w, 0, sizeof(w));
         w.params = params; w.points = points; w.n_points = n_points; w.out = u_out; w.ring_len = 1;
-        const long long tiles = (n_points + wide::Tile<128>::T - 1) / wide::Tile<128>::T;
-        const int grid = (int)(tiles < p->sm_count ? tiles : p->sm_count);
-        if (p->coupled)                        // u_out [n, k]
-            return launch_step(wide::wide128_coupled_forward_kernel, grid, 512, wide::Tile<128, true>::SMEM_BYTES, st, p->h, w);
-        return launch_step(wide::wide128_forward_kernel, grid, 512, wide::Tile<128>::SMEM_BYTES, st, p->h, w);
+        return launch_step(f.tile_fn, grid, f.threads, f.smem, st, p->h, w);
     }
     FwdArgs a;
     a.params = params; a.points = points; a.n_points = n_points; a.u_out = u_out;
     a.spill = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ws_spill_off(p));
-    a.rows_total = p->fwd_rows; a.row_scr = p->fwd_row_scr;
-    const int grid = grid_for(p, n_points, p->fwd_threads);
-    if (p->coupled) {
-        if (p->fwd_gmem) coupled_forward_kernel<true><<<grid, p->fwd_threads, p->fwd_smem_bytes, st>>>(p->h, a);
-        else             coupled_forward_kernel<false><<<grid, p->fwd_threads, p->fwd_smem_bytes, st>>>(p->h, a);
-    } else {
-        if (p->fwd_gmem) forward_kernel<true><<<grid, p->fwd_threads, p->fwd_smem_bytes, st>>>(p->h, a);
-        else             forward_kernel<false><<<grid, p->fwd_threads, p->fwd_smem_bytes, st>>>(p->h, a);
-    }
+    a.rows_total = f.rows; a.row_scr = f.row_scr;
+    f.fn<<<grid, f.threads, f.smem, st>>>(p->h, a);
     CUDA_TRY(cudaGetLastError());
     return PINN_OK;
 }
@@ -1033,12 +1015,12 @@ extern "C" int pinn_plan_info(const PinnPlan* p, PinnPlanInfo* info) {
     long long macs = 0;
     for (int l = 0; l < p->h.n_layers; ++l) macs += (long long)p->h.layer[l].n_in * p->h.layer[l].n_out;
     info->nf = p->h.nf; info->ns = p->h.ns; info->channels = C;
-    info->threads_per_cta = p->threads; info->ctas_per_sm = 1;
-    info->activations_in_smem = p->gmem ? 0 : 1;
-    info->tensor_core = p->wide ? (p->wide_kw == 128 ? 2 : 1) : 0;
-    info->small_batch_points = p->fn_small ? 8 * pinn::small::BP : 0;
-    info->smem_bytes = p->smem_bytes; info->regs_per_thread = p->regs; info->sm_count = p->sm_count;
-    info->rows_per_point = p->hs.rows_total;
+    info->threads_per_cta = p->step.threads; info->ctas_per_sm = 1;
+    info->activations_in_smem = p->step.state_in_smem ? 1 : 0;
+    info->tensor_core = p->step.tensor_core;
+    info->small_batch_points = p->small.solo ? 8 * pinn::small::BP : 0;
+    info->smem_bytes = p->step.smem; info->regs_per_thread = p->step.regs; info->sm_count = p->sm_count;
+    info->rows_per_point = p->step.plan.rows_total;
     info->flops_per_point = 6ll * C * macs;
     info->bytes_per_point = 4 * p->h.total;
     return PINN_OK;
