@@ -405,7 +405,8 @@ int pinn_multi_step_terms(const PinnPlan* plan, float* params, float* exp_avg, f
  * one CTA (multi-step kernel) or one cluster (cluster kernel) per member.  A PinnMember holds what differs between the
  * fits: their parameters, Adam state, mask, step tensors, step counter, loss ring, explicit batches (or NULL: sample
  * in-kernel with `cols` from the member's seed) and optimizer step count; everything else — plan, constraint terms,
- * batch size, k_steps, Adam hyper-parameters, ring_len, point weight — is shared.  Every member's result is bit-identical
+ * batch size, k_steps, Adam hyper-parameters (per member: pinn_multi_step_ensemble_adam below), ring_len, point
+ * weight — is shared.  Every member's result is bit-identical
  * to pinn_multi_step_terms on that member alone: the kernel and the cluster size are chosen by the same rule, and the
  * members never exchange anything.  The arguments are checked as pinn_multi_step_terms checks them, member by member;
  * n_members outside 1..PINN_MAX_MEMBERS, a null or misaligned (params: 16 bytes) member pointer: PINN_E_INVALID.
@@ -429,6 +430,23 @@ int pinn_multi_step_ensemble(const PinnPlan* plan, int n_members, const PinnMemb
                              int k_steps, float lr, float beta1, float beta2, float eps, float weight_decay,
                              int64_t ring_len, float point_weight, int n_terms, const PinnTerm* terms,
                              const PinnColumn* cols, void* stream);
+
+/*
+ * Hyper-parameter SWEEPS: pinn_multi_step_ensemble with Adam hyper-parameters of each member's own — member j steps with
+ * hyper[j] (host memory, n_members rows), the way torch.optim.Adam(lr=..., betas=(beta1, beta2), eps=..., weight_decay=...)
+ * would step that fit alone.  Everything else is checked and shared exactly as in pinn_multi_step_ensemble, and every
+ * member's result is bit-identical to pinn_multi_step_terms on that member alone with its own row; pinn_multi_step_ensemble
+ * is this call with every row equal to its shared arguments.  The rows are checked as torch.optim.Adam's constructor
+ * checks them: a null `hyper`, lr or eps non-finite or < 0, beta1 or beta2 outside [0, 1), weight_decay non-finite or
+ * < 0: PINN_E_INVALID, before anything launches.  The rows travel to the kernel by value with the member table.
+ */
+typedef struct PinnAdamHyper {
+    float lr, beta1, beta2, eps, weight_decay;
+} PinnAdamHyper;
+int pinn_multi_step_ensemble_adam(const PinnPlan* plan, int n_members, const PinnMember* members,
+                                  const PinnAdamHyper* hyper, int64_t n_points, int k_steps, int64_t ring_len,
+                                  float point_weight, int n_terms, const PinnTerm* terms, const PinnColumn* cols,
+                                  void* stream);
 
 /* Forward only: u = ansatz(net(x)) for explicit points — the work of Solver.predict
  * (model_torch.py:466-487) and of the `_forward` closure handed to constraints (:451-454).

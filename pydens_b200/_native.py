@@ -98,12 +98,20 @@ class PinnMember(C.Structure):
 
 MAX_MEMBERS = 128
 
+
+class PinnAdamHyper(C.Structure):
+    """ The Adam hyper-parameters of one member of pinn_multi_step_ensemble_adam. """
+    _fields_ = [('lr', C.c_float), ('beta1', C.c_float), ('beta2', C.c_float), ('eps', C.c_float),
+                ('weight_decay', C.c_float)]
+
+
 EXPORTS = ('pinn_last_error', 'pinn_abi_version', 'pinn_plan_create', 'pinn_plan_destroy',
            'pinn_workspace_bytes', 'pinn_out_floats', 'pinn_step', 'pinn_forward', 'pinn_sample',
            'pinn_record_loss', 'pinn_plan_info', 'pinn_comm_create', 'pinn_comm_connect', 'pinn_comm_destroy',
            'pinn_step_allreduce', 'pinn_comm_status', 'pinn_pipe_create', 'pinn_pipe_destroy', 'pinn_pipe_buffer',
            'pinn_pipe_step', 'pinn_pipe_finish', 'pinn_pipe_wait', 'pinn_pipe_sync', 'pinn_multi_step',
-           'pinn_multi_step_max_points', 'pinn_step_adam', 'pinn_multi_step_terms', 'pinn_multi_step_ensemble')
+           'pinn_multi_step_max_points', 'pinn_step_adam', 'pinn_multi_step_terms', 'pinn_multi_step_ensemble',
+           'pinn_multi_step_ensemble_adam')
 
 LIB_PATH = os.environ.get('PYDENS_B200_LIB') or os.path.join(os.path.dirname(os.path.abspath(__file__)), 'libpinn_b200.so')
 _lib = None
@@ -168,6 +176,9 @@ def load():
     lib.pinn_multi_step_ensemble.argtypes = [C.c_void_p, C.c_int, C.POINTER(PinnMember), C.c_int64, C.c_int,
                                              C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int64,
                                              C.c_float, C.c_int, C.POINTER(PinnTerm), C.POINTER(PinnColumn), C.c_void_p]
+    lib.pinn_multi_step_ensemble_adam.argtypes = [C.c_void_p, C.c_int, C.POINTER(PinnMember), C.POINTER(PinnAdamHyper),
+                                                  C.c_int64, C.c_int, C.c_int64, C.c_float, C.c_int, C.POINTER(PinnTerm),
+                                                  C.POINTER(PinnColumn), C.c_void_p]
     lib.pinn_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                  C.c_size_t, C.c_void_p]
     lib.pinn_sample.argtypes = [C.c_void_p, C.POINTER(PinnColumn), C.c_uint64, C.c_void_p, C.c_uint64,

@@ -812,9 +812,8 @@ struct MultiLaunch {
     int nc, smem;
 };
 
-static int multi_setup(PinnPlan* p, int64_t n_points, int k_steps, float lr, float beta1, float beta2, float eps,
-                       float weight_decay, int64_t ring_len, float point_weight, int n_terms, const PinnTerm* terms,
-                       MultiLaunch& L) {
+static int multi_setup(PinnPlan* p, int64_t n_points, int k_steps, int64_t ring_len, float point_weight, int n_terms,
+                       const PinnTerm* terms, MultiLaunch& L) {
     if (!p->multi.solo && !p->small.solo) return fail(PINN_E_UNSUPPORTED, "the persistent multi-step kernels do not fit this network in shared memory");
     if (n_terms < 0 || n_terms > PINN_MAX_TERMS || (n_terms > 0 && !terms))
         return fail(PINN_E_INVALID, "pinn_multi_step_terms: %d terms (0..%d)", n_terms, PINN_MAX_TERMS);
@@ -847,7 +846,6 @@ static int multi_setup(PinnPlan* p, int64_t n_points, int k_steps, float lr, flo
     L.plan = p->h;
     L.plan.n_slots = n_slots;                                       // the small kernel's scratch rows
     a.n_points = n_points; a.inv_n = point_weight; a.k_steps = k_steps;
-    a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = weight_decay;
     a.ring_len = ring_len;
     a.rows_total = rows;
     // batches of at most 128 points: the (point, unit)-parallel kernel (PINN_MULTI_KERNEL=tile forces the other one)
@@ -904,7 +902,7 @@ extern "C" int pinn_multi_step_terms(const PinnPlan* cp, float* params, float* e
     if (!p || !params || !exp_avg || !exp_avg_sq || !mask || !step_counter || !losses_ring)
         return fail(PINN_E_INVALID, "null argument");
     MultiLaunch L;
-    if (int rc = multi_setup(p, n_points, k_steps, lr, beta1, beta2, eps, weight_decay, ring_len, point_weight, n_terms, terms, L))
+    if (int rc = multi_setup(p, n_points, k_steps, ring_len, point_weight, n_terms, terms, L))
         return rc;
     if (n_step_tensors < 0) return fail(PINN_E_INVALID, "pinn_multi_step: n_step_tensors %d", n_step_tensors);
     if (!aligned16(params)) return fail(PINN_E_ALIGN, "params must be 16-byte aligned");
@@ -915,13 +913,14 @@ extern "C" int pinn_multi_step_terms(const PinnPlan* cp, float* params, float* e
     a.step_counter = reinterpret_cast<unsigned long long*>(step_counter);
     a.opt_step0 = opt_step0;
     a.losses_ring = losses_ring;
+    a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.weight_decay = weight_decay;
     return launch_persistent(L.k->solo, L, 1, stream);
 }
 
-extern "C" int pinn_multi_step_ensemble(const PinnPlan* cp, int n_members, const PinnMember* members, int64_t n_points,
-                                        int k_steps, float lr, float beta1, float beta2, float eps, float weight_decay,
-                                        int64_t ring_len, float point_weight, int n_terms, const PinnTerm* terms,
-                                        const PinnColumn* cols, void* stream) {
+// The launch of both ensemble entry points: `hyper` holds n_members rows, already checked.
+static int multi_step_ensemble(const PinnPlan* cp, int n_members, const PinnMember* members, const PinnAdamHyper* hyper,
+                               int64_t n_points, int k_steps, int64_t ring_len, float point_weight, int n_terms,
+                               const PinnTerm* terms, const PinnColumn* cols, void* stream) {
     PinnPlan* p = const_cast<PinnPlan*>(cp);
     if (!p || !members) return fail(PINN_E_INVALID, "null argument");
     if (n_members < 1 || n_members > PINN_MAX_MEMBERS)
@@ -936,15 +935,44 @@ extern "C" int pinn_multi_step_ensemble(const PinnPlan* cp, int n_members, const
         if (!m.points) sample = true;
     }
     static thread_local MultiLaunch L;                               // 13 KB: off the stack
-    static thread_local DevMembers table;                            // 10 KB
-    if (int rc = multi_setup(p, n_points, k_steps, lr, beta1, beta2, eps, weight_decay, ring_len, point_weight, n_terms, terms, L))
+    static thread_local DevMembers table;                            // 12.5 KB
+    if (int rc = multi_setup(p, n_points, k_steps, ring_len, point_weight, n_terms, terms, L))
         return rc;
     if (!L.k->ensemble)
         return fail(PINN_E_UNSUPPORTED, "the ensemble form of the persistent kernel does not fit this network");
     if (sample) { int rc = resolve_cols(p, cols, L.plan.cols); if (rc) return rc; }
     memset(&table, 0, sizeof(table));
     memcpy(table.m, members, sizeof(PinnMember) * (size_t)n_members);
+    memcpy(table.h, hyper, sizeof(PinnAdamHyper) * (size_t)n_members);
     return launch_persistent(L.k->ensemble, L, n_members, stream, table);
+}
+
+static bool finite_nonneg(float x) { return x >= 0.0f && x <= 3.4028235e38f; }   // false for NaN and inf
+
+extern "C" int pinn_multi_step_ensemble_adam(const PinnPlan* plan, int n_members, const PinnMember* members,
+                                             const PinnAdamHyper* hyper, int64_t n_points, int k_steps, int64_t ring_len,
+                                             float point_weight, int n_terms, const PinnTerm* terms,
+                                             const PinnColumn* cols, void* stream) {
+    if (!hyper) return fail(PINN_E_INVALID, "pinn_multi_step_ensemble_adam: null hyper");
+    for (int j = 0; j < n_members && j < PINN_MAX_MEMBERS; ++j) {   // torch.optim.Adam's checks, finite values only
+        const PinnAdamHyper& h = hyper[j];
+        if (!finite_nonneg(h.lr) || !(h.beta1 >= 0.0f && h.beta1 < 1.0f) || !(h.beta2 >= 0.0f && h.beta2 < 1.0f) ||
+            !finite_nonneg(h.eps) || !finite_nonneg(h.weight_decay))
+            return fail(PINN_E_INVALID, "member %d: lr %g, betas (%g, %g), eps %g, weight_decay %g (lr, eps, weight_decay "
+                        "finite and >= 0, betas in [0, 1))", j, h.lr, h.beta1, h.beta2, h.eps, h.weight_decay);
+    }
+    return multi_step_ensemble(plan, n_members, members, hyper, n_points, k_steps, ring_len, point_weight, n_terms, terms,
+                               cols, stream);
+}
+
+extern "C" int pinn_multi_step_ensemble(const PinnPlan* plan, int n_members, const PinnMember* members, int64_t n_points,
+                                        int k_steps, float lr, float beta1, float beta2, float eps, float weight_decay,
+                                        int64_t ring_len, float point_weight, int n_terms, const PinnTerm* terms,
+                                        const PinnColumn* cols, void* stream) {
+    static thread_local PinnAdamHyper rows[PINN_MAX_MEMBERS];
+    for (int j = 0; j < PINN_MAX_MEMBERS; ++j) rows[j] = PinnAdamHyper{lr, beta1, beta2, eps, weight_decay};
+    return multi_step_ensemble(plan, n_members, members, rows, n_points, k_steps, ring_len, point_weight, n_terms, terms,
+                               cols, stream);
 }
 
 extern "C" int pinn_multi_step(const PinnPlan* p, float* params, float* exp_avg, float* exp_avg_sq, const float* mask,

@@ -62,9 +62,10 @@ __host__ __device__ inline Layout make_layout(const DevPlan& P) {
     return L;
 }
 
-// The body of both forms: the fields of `mb` (MultiArgs itself, or one row of the member table) are the fit's own state.
-template <int NF, int NS, class MB>
-__device__ __forceinline__ void small_step_body(const DevPlan& P, const MultiArgs& a, const MB& mb) {
+// The body of both forms: the fields of `mb` (MultiArgs itself, or one row of the member table) are the fit's own state,
+// and those of `hy` (MultiArgs itself, or the member's row of hyper-parameters) its Adam hyper-parameters.
+template <int NF, int NS, class MB, class HY>
+__device__ __forceinline__ void small_step_body(const DevPlan& P, const MultiArgs& a, const MB& mb, const HY& hy) {
     constexpr int C = 1 + NF + NS;
     extern __shared__ __align__(16) float smem[];
     const int tid = threadIdx.x, lane = tid & 31;
@@ -121,9 +122,9 @@ __device__ __forceinline__ void small_step_body(const DevPlan& P, const MultiArg
         for (int i = tid; i < n_out_floats; i += NT) g[i] = 0.0f;
         // Adam's bias corrections do not depend on the gradient: computed here, off the critical path
         const float t_opt = mb.opt_step0 + (float)(s + 1);
-        const float bc1 = 1.0f - powf(a.beta1, t_opt);
-        const float bc2_sqrt = sqrtf(1.0f - powf(a.beta2, t_opt));
-        const float step_size = a.lr / bc1;
+        const float bc1 = 1.0f - powf(hy.beta1, t_opt);
+        const float bc2_sqrt = sqrtf(1.0f - powf(hy.beta2, t_opt));
+        const float step_size = hy.lr / bc1;
         __syncthreads();
 
         // ---- forward: layer l over (output unit j, point p) pairs ------------------------------------------------
@@ -344,10 +345,10 @@ __device__ __forceinline__ void small_step_body(const DevPlan& P, const MultiArg
                 if (mb.mask[i] != 0.0f) {
                     float gi = gsum[i];
                     const float pv = flat[i];
-                    if (a.weight_decay != 0.0f) gi = fmaf(a.weight_decay, pv, gi);
-                    const float m1 = fmaf(1.0f - a.beta1, gi - mom1[i], mom1[i]);
-                    const float m2 = fmaf(a.beta2, mom2[i], (1.0f - a.beta2) * gi * gi);
-                    flat[i] = pv - step_size * m1 / (sqrtf(m2) / bc2_sqrt + a.eps);
+                    if (hy.weight_decay != 0.0f) gi = fmaf(hy.weight_decay, pv, gi);
+                    const float m1 = fmaf(1.0f - hy.beta1, gi - mom1[i], mom1[i]);
+                    const float m2 = fmaf(hy.beta2, mom2[i], (1.0f - hy.beta2) * gi * gi);
+                    flat[i] = pv - step_size * m1 / (sqrtf(m2) / bc2_sqrt + hy.eps);
                     mom1[i] = m1; mom2[i] = m2;
                 }
             }
@@ -366,16 +367,18 @@ __device__ __forceinline__ void small_step_body(const DevPlan& P, const MultiArg
 
 template <int NF, int NS>
 __global__ void __launch_bounds__(NT, 1) small_step_kernel(const __grid_constant__ DevPlan P, const __grid_constant__ MultiArgs a) {
-    small_step_body<NF, NS>(P, a, a);
+    small_step_body<NF, NS>(P, a, a, a);
 }
 
-// The ensemble form (pinn_multi_step_ensemble): cluster c trains member c of the table.  Its CTAs exchange their
-// partials with each other only, in rank order, so each member's steps are those of its solo launch at the same
-// cluster size.
+// The ensemble form (pinn_multi_step_ensemble_adam): cluster c trains member c of the table with its Adam
+// hyper-parameters m.h[c].  Its CTAs exchange their partials with each other only, in rank order, so each member's
+// steps are those of its solo launch at the same cluster size.
 template <int NF, int NS>
 __global__ void __launch_bounds__(NT, 1) small_step_ensemble_kernel(const __grid_constant__ DevPlan P, const __grid_constant__ MultiArgs a,
                                                                     const __grid_constant__ DevMembers m) {
-    small_step_body<NF, NS>(P, a, m.m[blockIdx.x / cg::this_cluster().num_blocks()]);
+    const unsigned c = blockIdx.x / cg::this_cluster().num_blocks();
+    const PinnAdamHyper h = m.h[c];               // once, at entry: not an indexed parameter load per Adam element
+    small_step_body<NF, NS>(P, a, m.m[c], h);
 }
 
 }  // namespace small

@@ -573,17 +573,21 @@ struct MultiArgs {
 };
 // kernel parameters are limited to 32764 bytes (CUDA 12.1+ on Hopper); 16 bytes for the alignment of the second one
 static_assert(sizeof(DevPlan) + sizeof(MultiArgs) + 16 <= 32764, "DevPlan + MultiArgs exceed the kernel-parameter limit");
-// The member table of the ensemble form: what differs between the fits of an ensemble (the MultiArgs fields of the same
-// names are unused there).  A third __grid_constant__ parameter, read in place by the member's CTAs.
+// The member table of the ensemble form: what differs between the fits of an ensemble, their state and their Adam
+// hyper-parameters (the MultiArgs fields of the same names are unused there).  A third __grid_constant__ parameter, read
+// in place by the member's CTAs.
 struct DevMembers {
     PinnMember m[PINN_MAX_MEMBERS];
+    PinnAdamHyper h[PINN_MAX_MEMBERS];   // row b: the Adam of member b (pinn_multi_step_ensemble_adam)
 };
+// 13 344 + 12 800 = 26 144 bytes
 static_assert(sizeof(DevPlan) + sizeof(MultiArgs) + sizeof(DevMembers) + 32 <= 32764,
               "DevPlan + MultiArgs + the member table exceed the kernel-parameter limit");
 
-// The body of both forms: the fields of `mb` (MultiArgs itself, or one row of the member table) are the fit's own state.
-template <int NF, int NS, int JF, class MB>
-__device__ __forceinline__ void multi_step_body(const DevPlan& P, const MultiArgs& a, const MB& mb) {
+// The body of both forms: the fields of `mb` (MultiArgs itself, or one row of the member table) are the fit's own state,
+// and those of `hy` (MultiArgs itself, or the member's row of hyper-parameters) its Adam hyper-parameters.
+template <int NF, int NS, int JF, class MB, class HY>
+__device__ __forceinline__ void multi_step_body(const DevPlan& P, const MultiArgs& a, const MB& mb, const HY& hy) {
     extern __shared__ __align__(16) float smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
     const int n_out_floats = P.n_params + 4;
@@ -660,19 +664,19 @@ __device__ __forceinline__ void multi_step_body(const DevPlan& P, const MultiArg
         __syncthreads();
         // fold the warps in warp order, then Adam on the flat copy
         const float t_opt = mb.opt_step0 + (float)(s + 1);
-        const float bc1 = 1.0f - powf(a.beta1, t_opt);
-        const float bc2_sqrt = sqrtf(1.0f - powf(a.beta2, t_opt));
-        const float step_size = a.lr / bc1;
+        const float bc1 = 1.0f - powf(hy.beta1, t_opt);
+        const float bc2_sqrt = sqrtf(1.0f - powf(hy.beta2, t_opt));
+        const float step_size = hy.lr / bc1;
         for (int i = tid; i < n_out_floats; i += blockDim.x) {
             float g = 0.0f;
             for (int w = 0; w < nwarps; ++w) g += wacc_all[w * n_out_floats + i];
             gsum[i] = g;
             if (i < P.n_params && mb.mask[i] != 0.0f) {
                 float pv = flat[i];
-                if (a.weight_decay != 0.0f) g = fmaf(a.weight_decay, pv, g);
-                const float m1 = fmaf(1.0f - a.beta1, g - mom1[i], mom1[i]);
-                const float m2 = fmaf(a.beta2, mom2[i], (1.0f - a.beta2) * g * g);
-                const float denom = sqrtf(m2) / bc2_sqrt + a.eps;
+                if (hy.weight_decay != 0.0f) g = fmaf(hy.weight_decay, pv, g);
+                const float m1 = fmaf(1.0f - hy.beta1, g - mom1[i], mom1[i]);
+                const float m2 = fmaf(hy.beta2, mom2[i], (1.0f - hy.beta2) * g * g);
+                const float denom = sqrtf(m2) / bc2_sqrt + hy.eps;
                 flat[i] = pv - step_size * m1 / denom;
                 mom1[i] = m1; mom2[i] = m2;
             }
@@ -702,15 +706,17 @@ __device__ __forceinline__ void multi_step_body(const DevPlan& P, const MultiArg
 
 template <int NF, int NS, int MAXT, int JF>
 __global__ void __launch_bounds__(MAXT, 1) multi_step_kernel(const __grid_constant__ DevPlan P, const __grid_constant__ MultiArgs a) {
-    multi_step_body<NF, NS, JF>(P, a, a);
+    multi_step_body<NF, NS, JF>(P, a, a, a);
 }
 
-// The ensemble form (pinn_multi_step_ensemble): CTA b trains member b of the table, with the plan, the terms and the
-// Adam hyper-parameters of `a`; the members share nothing, so each one's steps are those of its solo launch.
+// The ensemble form (pinn_multi_step_ensemble_adam): CTA b trains member b of the table with its Adam hyper-parameters
+// m.h[b], and with the plan and the terms of `a`; the members share nothing, so each one's steps are those of its solo
+// launch.
 template <int NF, int NS, int MAXT, int JF>
 __global__ void __launch_bounds__(MAXT, 1) multi_step_ensemble_kernel(const __grid_constant__ DevPlan P, const __grid_constant__ MultiArgs a,
                                                                       const __grid_constant__ DevMembers m) {
-    multi_step_body<NF, NS, JF>(P, a, m.m[blockIdx.x]);
+    const PinnAdamHyper h = m.h[blockIdx.x];      // once, at entry: not an indexed parameter load per Adam element
+    multi_step_body<NF, NS, JF>(P, a, m.m[blockIdx.x], h);
 }
 
 typedef void (*MultiKernelFn)(const DevPlan, const MultiArgs);

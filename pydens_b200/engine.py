@@ -162,9 +162,10 @@ def run_persistent(engines, opts, samplers, terms, niters, batch_size, k, table)
     """ `niters` optimizer steps of every engine's fit, `k` per launch of the persistent multi-step kernels: the
     reference loop model_torch.py:426-464 with optimizer.step() inside the kernel, constraint terms included.  One fit
     runs on the solo kernels (pinn_multi_step_terms) unless `table` is set; with `table` the fits are members of
-    pinn_multi_step_ensemble, at most MAX_MEMBERS per launch.  `samplers` has one sampler per fit: all in-kernel with
-    the same columns, or all on the host.  Returns None, or the library's message when it refused the first launch
-    with PINN_E_UNSUPPORTED (no step has been taken then). """
+    pinn_multi_step_ensemble_adam, at most MAX_MEMBERS per launch, each with the Adam hyper-parameters of its own
+    optimizer.  `samplers` has one sampler per fit: all in-kernel with the same columns, or all on the host.  Returns
+    None, or the library's message when it refused the first launch with PINN_E_UNSUPPORTED (no step has been taken
+    then). """
     e0 = engines[0]
     lib, total, ring_len = e0.lib, e0.solver.model.total, e0.ring.numel()
     # point weights: the mean of model_torch.py:448 over the batch and over every constraint's own points, or 1
@@ -178,8 +179,10 @@ def run_persistent(engines, opts, samplers, terms, niters, batch_size, k, table)
     point_weight = 1.0 if total_sum else 1.0 / batch_size
     M = len(engines)
     members = (_native.PinnMember * M)()
+    hyper = (_native.PinnAdamHyper * M)()
     starts, step0 = [], []
-    for mb, eng, opt in zip(members, engines, opts):
+    for mb, hy, eng, opt in zip(members, hyper, engines, opts):
+        hy.lr, (hy.beta1, hy.beta2), hy.eps, hy.weight_decay = adam_hyper(opt)
         eng._adopt_optimizer()
         mask = eng._bind_adam_state(opt)
         m, v, steps, _ = eng._adam_flat
@@ -193,7 +196,7 @@ def run_persistent(engines, opts, samplers, terms, niters, batch_size, k, table)
     host = cols_key is None
     lr, (b1, b2), eps, wd = adam_hyper(opts[0])
     stream = e0._stream()
-    size = C.sizeof(_native.PinnMember)
+    size, hsize = C.sizeof(_native.PinnMember), C.sizeof(_native.PinnAdamHyper)
     vals = np.empty((M, niters), dtype=np.float32)
 
     def drain(lo, hi):
@@ -219,11 +222,12 @@ def run_persistent(engines, opts, samplers, terms, niters, batch_size, k, table)
             mb.opt_step0 = s0 + done
         for lo in range(0, M, _native.MAX_MEMBERS):
             if table:
-                rc = lib.pinn_multi_step_ensemble(
+                rc = lib.pinn_multi_step_ensemble_adam(
                     e0.plan, min(_native.MAX_MEMBERS, M - lo),
-                    C.cast(C.addressof(members) + lo * size, C.POINTER(_native.PinnMember)), C.c_int64(batch_size),
-                    C.c_int(kk), C.c_float(lr), C.c_float(b1), C.c_float(b2), C.c_float(eps), C.c_float(wd),
-                    C.c_int64(ring_len), C.c_float(point_weight), C.c_int(len(terms)), term_arr, cols, stream)
+                    C.cast(C.addressof(members) + lo * size, C.POINTER(_native.PinnMember)),
+                    C.cast(C.addressof(hyper) + lo * hsize, C.POINTER(_native.PinnAdamHyper)), C.c_int64(batch_size),
+                    C.c_int(kk), C.c_int64(ring_len), C.c_float(point_weight), C.c_int(len(terms)), term_arr, cols,
+                    stream)
             else:
                 mb = members[0]
                 rc = lib.pinn_multi_step_terms(

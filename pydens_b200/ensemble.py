@@ -5,15 +5,17 @@ variable, or solve one equation for many values of a frozen coefficient.  Each s
 cluster of at most 8 CTAs; `fit_ensemble` puts up to PINN_MAX_MEMBERS of them into one launch
 (pinn_multi_step_ensemble), one CTA or cluster per member.  It means exactly "call `s.fit(...)` on every solver": every
 member keeps its own seed, optimizer state, frozen mask, loss list and step counter, and its result is bit-identical to
-its solo fit.
+its solo fit.  Each member may also take its own Adam hyper-parameters (a learning-rate sweep: `lr=[...]`), which the
+kernels read from the member's row of the table (pinn_multi_step_ensemble_adam).
 """
 import warnings
 
+import numpy as np
 from torch import nn
 
 from . import _native
-from .engine import (_AUTO_PERSISTENT_STEPS, _dist, adam_hyper, adam_steps_equal, auto_persistent, plain_adam,
-                     run_persistent, sampler_columns)
+from .engine import (_AUTO_PERSISTENT_STEPS, _dist, adam_steps_equal, auto_persistent, plain_adam, run_persistent,
+                     sampler_columns)
 
 # what each part of the problem's spec describes, for the error that names the difference between two members
 _SPEC_PARTS = (
@@ -60,6 +62,27 @@ def member_samplers(sampler, n):
     return [sampler] * n
 
 
+def _per_member(v):
+    return isinstance(v, (list, tuple)) or (isinstance(v, np.ndarray) and v.ndim > 0)
+
+
+def member_hyper(n, lr, kwargs):
+    """ Each member's (lr, optimizer kwargs): `lr`, `eps` and `weight_decay` are one value for all or a sequence of n,
+    `betas` one pair for all or a sequence of n pairs.  Raises ValueError for a sequence of another length. """
+    def spread(name, v, pairs=False):
+        if not _per_member(v) or (pairs and not (len(v) and _per_member(v[0]))):
+            return [v] * n
+        if len(v) != n:
+            raise ValueError('fit_ensemble: %d values of %s for %d solvers' % (len(v), name, n))
+        return list(v)
+    kws = [dict(kwargs) for _ in range(n)]
+    for name in ('betas', 'eps', 'weight_decay'):
+        if name in kwargs:
+            for kw, v in zip(kws, spread(name, kwargs[name], pairs=name == 'betas')):
+                kw[name] = v
+    return spread('lr', lr), kws
+
+
 def fit_ensemble(solvers, niters, batch_size, sampler=None, loss_terms='equation', optimizer='Adam',
                  criterion=nn.MSELoss(), lr=0.005, steps_per_launch=None, **kwargs):
     """ `s.fit(niters, batch_size, sampler, loss_terms, optimizer, criterion, lr, ...)` for every solver in `solvers`,
@@ -71,14 +94,20 @@ def fit_ensemble(solvers, niters, batch_size, sampler=None, loss_terms='equation
     sampler   None, one sampler shared by all members, or a list with one per member.  In-kernel samplers draw each
               member's batch from its own seed; a shared host sampler gives each member its batches in member order,
               launch by launch.
+    lr        one learning rate, or a sequence with one per member; so are `eps` and `weight_decay` among the optimizer
+              kwargs, and `betas` is one pair or a sequence of one pair per member.  Member j then fits as
+              `s.fit(..., lr=lr[j], betas=betas[j], ...)`, and its optimizer keeps its own settings for a later
+              `fit(optimizer=None)`.  With optimizer=None every member keeps its existing optimizer, whatever its
+              settings.
     Anything the persistent path cannot take fits the solvers one after another with their own `fit`, after one
     UserWarning giving the reason; decoupled weight decay (decoupled_weight_decay=True with weight_decay > 0) is one
-    such fit, it runs on torch's Adam.  Raises ValueError for the same Solver twice, solvers on different devices, or
-    solvers whose problems differ.
+    such fit, it runs on torch's Adam.  Raises ValueError for the same Solver twice, solvers on different devices,
+    solvers whose problems differ, or a per-member sequence whose length is not the number of solvers.
     """
     solvers = list(solvers)
     check_members(solvers)
     samplers = member_samplers(sampler, len(solvers))
+    lrs, kws = member_hyper(len(solvers), lr, kwargs)
     loss_terms = tuple(loss_terms) if isinstance(loss_terms, (tuple, list)) else (loss_terms,)
     why = None
     if niters > 0:
@@ -88,14 +117,15 @@ def fit_ensemble(solvers, niters, batch_size, sampler=None, loss_terms='equation
             return
         warnings.warn('pydens_b200.fit_ensemble: fitting the solvers one after another (%s)' % why, UserWarning,
                       stacklevel=2)
-    if steps_per_launch is not None:
-        kwargs['steps_per_launch'] = steps_per_launch
-    for s, smp in zip(solvers, samplers):
-        s.fit(niters, batch_size, smp, list(loss_terms), optimizer, criterion, lr, **dict(kwargs))
+    for s, smp, lr_j, kw in zip(solvers, samplers, lrs, kws):
+        if steps_per_launch is not None:
+            kw['steps_per_launch'] = steps_per_launch
+        s.fit(niters, batch_size, smp, list(loss_terms), optimizer, criterion, lr_j, **kw)
 
 
 def _fit_together(solvers, niters, batch_size, samplers, loss_terms, optimizer, criterion, lr, steps_per_launch, kwargs):
-    """ The ensemble fit, or the reason it cannot run (nothing has been trained then). """
+    """ The ensemble fit, each member with the optimizer of its own values of `lr` and `kwargs` (member_hyper), or the
+    reason it cannot run (nothing has been trained then). """
     if _dist() is not None:
         return 'torch.distributed runs several ranks'
     engines = []
@@ -135,15 +165,13 @@ def _fit_together(solvers, niters, batch_size, samplers, loss_terms, optimizer, 
     if len({sampler_columns(smp, total)[0] for smp in samplers}) > 1:
         return 'the members\' samplers differ in their in-kernel columns, or some sample on the host'
     opts = []
-    for eng in engines:
-        opt, _ = eng._optimizer_for(optimizer, lr, dict(kwargs))
+    for eng, lr_j, kw in zip(engines, *member_hyper(len(solvers), lr, kwargs)):
+        opt, _ = eng._optimizer_for(optimizer, lr_j, kw)
         if not plain_adam(opt):
             return ('the optimizer is not plain torch.optim.Adam with one parameter group and L2 weight decay '
                     '(decoupled weight decay runs on torch\'s Adam)')
         if not adam_steps_equal(opt):
             return 'the optimizer has taken different numbers of steps for different parameters'
         opts.append(opt)
-    if len({adam_hyper(o) for o in opts}) > 1:
-        return 'the members\' Adam hyper-parameters differ'
     return run_persistent(engines, opts, samplers, terms[0], niters, batch_size, k, table=True)
 
