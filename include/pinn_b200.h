@@ -503,6 +503,69 @@ typedef struct PinnPlanInfo {
 } PinnPlanInfo;
 int pinn_plan_info(const PinnPlan* plan, PinnPlanInfo* info);
 
+/*
+ * L-BFGS ON THE DEVICE: torch.optim.LBFGS.step(closure) (torch 2.11, torch/optim/lbfgs.py) as a state machine whose
+ * state lives in one device buffer.  The caller evaluates the objective (pinn_step and whatever it adds to
+ * [grads | loss]) at `params`, then calls pinn_lbfgs_advance, which consumes that evaluation, writes into `params` the
+ * point of the next evaluation (or the step's final point) and sets *status (device int):
+ *   PINN_LBFGS_EVALUATE  evaluate again at `params` and call pinn_lbfgs_advance again (the same step goes on),
+ *   PINN_LBFGS_DONE      the step is finished: losses_ring[*step_counter % ring_len] = the loss of the step's first
+ *                        evaluation (what step(closure) returns; skipped when losses_ring is NULL); ++*step_counter.
+ * Every branch of torch's step is restated: the first iteration's d = -g and t = min(1, 1/|g|_1) lr, the ys > 1e-10
+ * memory update over a ring of history_size pairs, H_diag, the gtd > -tolerance_change break, the fixed step without
+ * re-evaluation on the last inner iteration, every exit test (opt_cond at entry, max_iter, max_eval, opt_cond,
+ * max|d t| <= tolerance_change, |loss - prev_loss| < tolerance_change), and _strong_wolfe with _cubic_interpolate
+ * (c1 = 1e-4, c2 = 0.9, max_ls = max_eval - evaluations so far).  Only entries with mask = 1 take part in any dot
+ * product, norm or update.  Dot products and scalars are fp64, vectors fp32; every reduction has a fixed order, so runs
+ * are bit-reproducible.  One CTA; stream-ordered, capturable, allocates nothing.  A zeroed state buffer of
+ * pinn_lbfgs_state_bytes(n_params, history_size) bytes is a fresh optimizer.  lr < 0, max_iter < 1, max_eval < 1,
+ * history_size < 1, line_search not 0 / 1, a null pointer: PINN_E_INVALID.
+ */
+#define PINN_LBFGS_DONE          0
+#define PINN_LBFGS_EVALUATE      1
+typedef struct PinnLbfgs {
+    double lr, tolerance_grad, tolerance_change;
+    int32_t max_iter, max_eval, history_size;
+    int32_t line_search;       /* 0: fixed step (line_search_fn=None), 1: 'strong_wolfe' */
+    const float* mask;         /* device [n_params]: 1 = in the optimizer, 0 = frozen or padding */
+    float* losses_ring;        /* device [ring_len], or NULL */
+    int64_t ring_len;
+    uint64_t* step_counter;    /* device step number (the in-kernel sampler's Philox step), += 1 per finished step */
+} PinnLbfgs;
+
+/*
+ * The state buffer: this header, then fp64 arrays, then fp32 vectors.  With S = history_size + 1 (ring slots: the
+ * pairs held plus the one the next pair is written to), nv = n_params rounded up to a multiple of 4:
+ *   offset PINN_LBFGS_HEADER_BYTES:  double sy[S][S]  (sy[p][q] = s_p . y_q, physical slots), yy[S][S],
+ *                                    sg[S], yg[S] (s_p . g, y_p . g of the last direction), al[S], cs[S], cy[S]
+ *                                    (torch's `al`, and d = hg g + sum_i cs[i] s_i + cy[i] y_i, logical order)
+ *   offset pinn_lbfgs_vector_offset(history_size), each nv floats:  0 d, 1 prev_flat_grad, 2 x (line-search base),
+ *                                    3..5 line-search gradient copies, 6..6+S-1 s slots, 6+S..6+2S-1 y slots.
+ * Pair i (0 = oldest) of the history sits in physical slot (ring_head + i) % S.
+ */
+#define PINN_LBFGS_HEADER_BYTES 512
+typedef struct PinnLbfgsState {
+    /* torch's state */
+    int64_t n_iter, func_evals;
+    double t, H_diag, prev_loss;
+    int32_t ring_count, ring_head;
+    /* the running step */
+    int32_t phase, cur_iter, current_evals, opt_cond, g_src, action, act_arg, act_eval;
+    double loss, first_loss, gtd, d_norm, gsum_g, hg;
+    /* _strong_wolfe */
+    int32_t ls_iter, ls_evals, max_ls, ls_done, ls_zoom, insuf, low, high, gp_ref, new_ref;
+    double t_prev, f_prev, gtd_prev, f_new, gtd_new;
+    double br_t[2], br_f[2], br_gtd[2];
+    int32_t br_g[2];
+    double ref_gmax[5];        /* max|g| of the gradients the state refers to: the evaluation, prev_flat_grad, copies */
+    /* results of the last vector pass */
+    double r_dot, r_max, r_l1;
+} PinnLbfgsState;
+size_t pinn_lbfgs_state_bytes(int64_t n_params, int history_size);
+size_t pinn_lbfgs_vector_offset(int history_size);
+int pinn_lbfgs_advance(const PinnLbfgs* cfg, int64_t n_params, float* params, const float* grads_and_loss,
+                       void* state, int* status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -105,13 +105,55 @@ class PinnAdamHyper(C.Structure):
                 ('weight_decay', C.c_float)]
 
 
+class PinnLbfgs(C.Structure):
+    """ The settings of pinn_lbfgs_advance: torch.optim.LBFGS's, the optimizer's mask and the loss ring. """
+    _fields_ = [('lr', C.c_double), ('tolerance_grad', C.c_double), ('tolerance_change', C.c_double),
+                ('max_iter', C.c_int32), ('max_eval', C.c_int32), ('history_size', C.c_int32), ('line_search', C.c_int32),
+                ('mask', C.c_void_p), ('losses_ring', C.c_void_p), ('ring_len', C.c_int64), ('step_counter', C.c_void_p)]
+
+
+class PinnLbfgsState(C.Structure):
+    """ The scalar header of an L-BFGS state buffer (include/pinn_b200.h). """
+    _fields_ = [('n_iter', C.c_int64), ('func_evals', C.c_int64), ('t', C.c_double), ('H_diag', C.c_double),
+                ('prev_loss', C.c_double), ('ring_count', C.c_int32), ('ring_head', C.c_int32),
+                ('phase', C.c_int32), ('cur_iter', C.c_int32), ('current_evals', C.c_int32), ('opt_cond', C.c_int32),
+                ('g_src', C.c_int32), ('action', C.c_int32), ('act_arg', C.c_int32), ('act_eval', C.c_int32),
+                ('loss', C.c_double), ('first_loss', C.c_double), ('gtd', C.c_double), ('d_norm', C.c_double),
+                ('gsum_g', C.c_double), ('hg', C.c_double),
+                ('ls_iter', C.c_int32), ('ls_evals', C.c_int32), ('max_ls', C.c_int32), ('ls_done', C.c_int32),
+                ('ls_zoom', C.c_int32), ('insuf', C.c_int32), ('low', C.c_int32), ('high', C.c_int32),
+                ('gp_ref', C.c_int32), ('new_ref', C.c_int32),
+                ('t_prev', C.c_double), ('f_prev', C.c_double), ('gtd_prev', C.c_double), ('f_new', C.c_double),
+                ('gtd_new', C.c_double), ('br_t', C.c_double * 2), ('br_f', C.c_double * 2), ('br_gtd', C.c_double * 2),
+                ('br_g', C.c_int32 * 2), ('ref_gmax', C.c_double * 5),
+                ('r_dot', C.c_double), ('r_max', C.c_double), ('r_l1', C.c_double)]
+
+
+LBFGS_HEADER_BYTES, LBFGS_DONE, LBFGS_EVALUATE = 512, 0, 1
+LBFGS_D, LBFGS_PG, LBFGS_X, LBFGS_RING = 0, 1, 2, 6        # vector slots of the state buffer
+
+
+def lbfgs_layout(n_params, history_size, itemsize=4):
+    """ Where the parts of an L-BFGS state buffer lie (include/pinn_b200.h): byte offsets of the fp64 arrays
+    (sy, yy: S x S; sg, yg, al, cs, cy: S), of the vectors (nv items each), nv, S and the total size. """
+    S = history_size + 1
+    nv = (n_params + 3) // 4 * 4
+    f64 = {}
+    off = LBFGS_HEADER_BYTES
+    for name, count in (('sy', S * S), ('yy', S * S), ('sg', S), ('yg', S), ('al', S), ('cs', S), ('cy', S)):
+        f64[name] = (off, count)
+        off += 8 * count
+    vec = (off + 255) // 256 * 256
+    return dict(f64=f64, vectors=vec, nv=nv, S=S, total=vec + itemsize * nv * (LBFGS_RING + 2 * S))
+
+
 EXPORTS = ('pinn_last_error', 'pinn_abi_version', 'pinn_plan_create', 'pinn_plan_destroy',
            'pinn_workspace_bytes', 'pinn_out_floats', 'pinn_step', 'pinn_forward', 'pinn_sample',
            'pinn_record_loss', 'pinn_plan_info', 'pinn_comm_create', 'pinn_comm_connect', 'pinn_comm_destroy',
            'pinn_step_allreduce', 'pinn_comm_status', 'pinn_pipe_create', 'pinn_pipe_destroy', 'pinn_pipe_buffer',
            'pinn_pipe_step', 'pinn_pipe_finish', 'pinn_pipe_wait', 'pinn_pipe_sync', 'pinn_multi_step',
            'pinn_multi_step_max_points', 'pinn_step_adam', 'pinn_multi_step_terms', 'pinn_multi_step_ensemble',
-           'pinn_multi_step_ensemble_adam')
+           'pinn_multi_step_ensemble_adam', 'pinn_lbfgs_state_bytes', 'pinn_lbfgs_vector_offset', 'pinn_lbfgs_advance')
 
 LIB_PATH = os.environ.get('PYDENS_B200_LIB') or os.path.join(os.path.dirname(os.path.abspath(__file__)), 'libpinn_b200.so')
 _lib = None
@@ -185,6 +227,12 @@ def load():
                                 C.c_uint64, C.c_int64, C.c_void_p, C.c_void_p]
     lib.pinn_record_loss.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
     lib.pinn_plan_info.argtypes = [C.c_void_p, C.POINTER(PinnPlanInfo)]
+    lib.pinn_lbfgs_state_bytes.restype = C.c_size_t
+    lib.pinn_lbfgs_state_bytes.argtypes = [C.c_int64, C.c_int]
+    lib.pinn_lbfgs_vector_offset.restype = C.c_size_t
+    lib.pinn_lbfgs_vector_offset.argtypes = [C.c_int]
+    lib.pinn_lbfgs_advance.argtypes = [C.POINTER(PinnLbfgs), C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p]
     if lib.pinn_abi_version() != ABI_VERSION:
         raise LibraryMissing('libpinn_b200.so ABI %d != binding ABI %d: rebuild' % (lib.pinn_abi_version(), ABI_VERSION))
     _lib = lib

@@ -203,6 +203,8 @@ struct PinnPlan {
 };
 
 extern "C" const char* pinn_last_error(void) { return g_err; }
+// the error message of the other build units (pinn_lbfgs.cu)
+int pinn_fail_message(int code, const char* msg) { return fail(code, "%s", msg); }
 extern "C" int pinn_abi_version(void) { return PINN_ABI_VERSION; }
 
 // The dynamic shared-memory limit is an attribute of the KERNEL, shared by every plan that uses the same

@@ -601,6 +601,12 @@ class FusedEngine:
         # _AUTO_PERSISTENT_STEPS optimizer steps per launch (same math, same loss log; PYDENS_B200_AUTO_PERSISTENT=0
         # keeps one launch per step).  An explicit steps_per_launch takes precedence.
         requested = steps_per_launch > 0
+        if type(opt) is torch.optim.LBFGS and len(opt.param_groups) == 1:
+            if requested:
+                warnings.warn('pydens_b200: steps_per_launch ignored (L-BFGS runs one evaluation per launch)',
+                              stacklevel=3)
+            self._fit_lbfgs(niters, batch_size, sampler, loss_terms, criterion, opt)
+            return
         if not requested and auto_persistent(niters, batch_size, self.info):
             steps_per_launch = _AUTO_PERSISTENT_STEPS
         if steps_per_launch > 0 and niters > 0:
@@ -617,11 +623,11 @@ class FusedEngine:
                                  self.lib.pinn_multi_step_max_points(self.plan)), stacklevel=3)
         self._fit_stepwise(niters, batch_size, sampler, loss_terms, criterion, opt, opt_ready)
 
-    def _fit_stepwise(self, niters, batch_size, sampler, loss_terms, criterion, opt, opt_ready):
-        """ One launch of the step kernel per optimizer step, with the constraint launches, autograd's constraints and
-        torch's optimizer (or the Adam in the step kernel's tail); captured in CUDA graphs where possible. """
+    def _eval_setup(self, niters, batch_size, sampler, loss_terms, criterion):
+        """ What an evaluation of the objective (_evaluate) needs for a fit: the terms, this rank's share of the batch,
+        the point weight, the sampler's columns; points every parameter's .grad at its view of `out`.  None for a fit of
+        no step (after the batch check, before anything is rebound). """
         solver = self.solver
-        self._adopt_optimizer()
         nums = solver._constraint_numbers(loss_terms)
         eq_term = 'equation' in loss_terms                # reference :448: the equation term is optional (:382-389)
         fused_constraints = [e for e in (self._constraint_plan(n) for n in nums) if e is not None]
@@ -638,8 +644,7 @@ class FusedEngine:
         inv_n = 1.0 if self._sum_reduction() else 1.0 / float(batch_size)
         total = solver.model.total
         if niters <= 0:
-            return
-
+            return None
         # every parameter's .grad must be the view of `out` (a previous zero_grad may have dropped it)
         for p, o in self.entries:
             if p.grad is None or p.grad.data_ptr() != self.out.data_ptr() + 4 * o:
@@ -649,6 +654,22 @@ class FusedEngine:
         # reference does (model_torch.py:428)
         entry_ids = {id(p) for p, _ in self.entries}
         stray_params = [p for p in solver.model.parameters() if id(p) not in entry_ids]
+        cols_key, cols = sampler_columns(sampler, total)
+        return dict(eq_term=eq_term, cols_key=cols_key, cols=cols, local_n=local_n, inv_n=inv_n,
+                    point_offset=point_offset, dist=dist, fused_constraints=fused_constraints, fused_nums=fused_nums,
+                    nums=nums, stray_params=stray_params, batch_size=batch_size, total=total, criterion=criterion)
+
+    def _fit_stepwise(self, niters, batch_size, sampler, loss_terms, criterion, opt, opt_ready):
+        """ One launch of the step kernel per optimizer step, with the constraint launches, autograd's constraints and
+        torch's optimizer (or the Adam in the step kernel's tail); captured in CUDA graphs where possible. """
+        solver = self.solver
+        self._adopt_optimizer()
+        ev = self._eval_setup(niters, batch_size, sampler, loss_terms, criterion)
+        if ev is None:
+            return
+        eq_term, fused_constraints, fused_nums, nums = ev['eq_term'], ev['fused_constraints'], ev['fused_nums'], ev['nums']
+        dist, local_n, point_offset, inv_n, total = ev['dist'], ev['local_n'], ev['point_offset'], ev['inv_n'], ev['total']
+        stray_params = ev['stray_params']
 
         # optimizer.step() inside the step kernel (pinn_step_adam) whenever the optimizer is the plain torch Adam this
         # engine builds and nothing has to touch the gradient between the kernel and the update
@@ -672,37 +693,15 @@ class FusedEngine:
             # all-reduce waits only a bounded time for its peers, so line the ranks up first
             dist.barrier()
 
-        cols_key, cols = sampler_columns(sampler, total)
+        cols_key, cols = ev['cols_key'], ev['cols']
         solver.model.train()
-        loss_idx = self.n_params
         ring_ptr, ring_len = self.ring.data_ptr(), self.ring.numel()
 
         def one_step(points=None, full_points=None):
             if fused_adam:
                 self._step_adam(points, cols, local_n, inv_n, point_offset, adam, allreduce=dist is not None)
                 return
-            if eq_term:
-                self._step(points, cols, local_n, inv_n, point_offset, allreduce=dist is not None)
-                if dist is not None and self.comm is None:
-                    dist.all_reduce(self.out)          # no peer-memory path: NCCL sums [grads | loss]
-            else:
-                self.out.zero_()                       # loss_terms without 'equation': the constraint terms alone
-            for entry in fused_constraints:            # after the all-reduce: every rank adds the same term
-                self._constraint_step(entry)
-            if nums:
-                # constraints that stay on autograd see the step's own batch — the WHOLE global batch, identical
-                # on every rank (so that every replica adds the same gradient) and with requires_grad set, as the
-                # reference hands them to the constraint (model_torch.py:436, :451-457)
-                if full_points is not None:
-                    batch = full_points
-                else:                                  # in-kernel sampler: replay the batch the kernel just drew
-                    batch = self.sample(batch_size, cols, point_offset=0)
-                xs = [batch[:, k:k + 1].clone().requires_grad_() for k in range(total)]
-                for p in stray_params:
-                    p.grad = None
-                closs = solver._constraint_loss(nums, xs, criterion)
-                closs.backward()
-                self.out[loss_idx] += closs.detach()
+            self._evaluate(ev, points, full_points)
             opt.step()
             _native.check(self.lib.pinn_record_loss(self.plan, C.c_void_p(self.out.data_ptr()),
                                                     C.c_void_p(ring_ptr), C.c_int64(ring_len),
@@ -716,6 +715,147 @@ class FusedEngine:
             vals = self._loop_host_batches(niters, batch_size, local_n, point_offset, sampler, one_step, graphs_ok,
                                            ('host', batch_size, local_n, fused_nums, adam_key), nums, dist)
         self._end_stepwise(vals, dist)
+
+    def _evaluate(self, ev, points=None, full_points=None):
+        """ The objective of a step into [grads | loss] (`out`): the equation launch (or zeros), the all-reduce, the
+        fused constraint launches and the constraints autograd adds, on the step's batch (`points`: this rank's rows of
+        an explicit batch, None: the in-kernel sampler's; `full_points`: the whole explicit batch, for autograd). """
+        dist = ev['dist']
+        if ev['eq_term']:
+            self._step(points, ev['cols'], ev['local_n'], ev['inv_n'], ev['point_offset'], allreduce=dist is not None)
+            if dist is not None and self.comm is None:
+                dist.all_reduce(self.out)          # no peer-memory path: NCCL sums [grads | loss]
+        else:
+            self.out.zero_()                       # loss_terms without 'equation': the constraint terms alone
+        for entry in ev['fused_constraints']:      # after the all-reduce: every rank adds the same term
+            self._constraint_step(entry)
+        if ev['nums']:
+            # constraints that stay on autograd see the step's own batch — the WHOLE global batch, identical
+            # on every rank (so that every replica adds the same gradient) and with requires_grad set, as the
+            # reference hands them to the constraint (model_torch.py:436, :451-457)
+            if full_points is not None:
+                batch = full_points
+            else:                                  # in-kernel sampler: replay the batch the kernel just drew
+                batch = self.sample(ev['batch_size'], ev['cols'], point_offset=0)
+            total = ev['total']
+            xs = [batch[:, k:k + 1].clone().requires_grad_() for k in range(total)]
+            for p in ev['stray_params']:
+                p.grad = None
+            closs = self.solver._constraint_loss(ev['nums'], xs, ev['criterion'])
+            closs.backward()
+            self.out[self.n_params] += closs.detach()
+
+    # ------------------------------------------------------------------------------------------
+    # L-BFGS: torch.optim.LBFGS.step(closure) with the update on the device (pinn_lbfgs_advance)
+    def _lbfgs_bind(self, opt):
+        """ The device state of `opt` -> (PinnLbfgs settings, state buffer, mask, torch-order index).  A state torch
+        left in opt.state (its own steps, or a write-back that torch has stepped past since) is imported first. """
+        g = opt.param_groups[0]
+        m = int(g['history_size'])
+        params = list(g['params'])
+        pos = {id(p): o for p, o in self.entries}
+        idx = torch.cat([torch.arange(pos[id(p)], pos[id(p)] + p.numel(), device=self.device) for p in params])
+        mask = torch.zeros(self.n_params, dtype=torch.float32, device=self.device)
+        mask[idx] = 1.0
+        nbytes = self.lib.pinn_lbfgs_state_bytes(self.n_params, m)
+        cur = getattr(self, '_lbfgs', None)
+        if cur is None or cur['opt'] is not opt or cur['state'].numel() != nbytes or not cur['fresh'](opt):
+            state = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
+            cur = dict(opt=opt, state=state, m=m, idx=idx, fresh=lambda o: False)
+            st = opt.state.get(params[0])
+            if st and 'n_iter' in st:
+                lbfgs_import(state, st, idx, self.n_params, m)
+            self._lbfgs = cur
+        cfg = _native.PinnLbfgs(lr=float(g['lr']), tolerance_grad=float(g['tolerance_grad']),
+                                tolerance_change=float(g['tolerance_change']), max_iter=int(g['max_iter']),
+                                max_eval=int(g['max_eval']), history_size=m,
+                                line_search=int(g['line_search_fn'] == 'strong_wolfe'), mask=mask.data_ptr(),
+                                losses_ring=self.ring.data_ptr(), ring_len=self.ring.numel(),
+                                step_counter=self.step_counter.data_ptr())
+        if g['line_search_fn'] not in (None, 'strong_wolfe'):
+            raise RuntimeError("only 'strong_wolfe' is supported")
+        return cfg, cur, mask
+
+    def _fit_lbfgs(self, niters, batch_size, sampler, loss_terms, criterion, opt):
+        """ `niters` L-BFGS steps: per evaluation of the objective (_evaluate, on the step's one batch) one
+        pinn_lbfgs_advance and a read of its 4-byte status; the step counter (the in-kernel sampler's Philox step)
+        moves only when the kernel finishes a step.  The device state is written back into opt.state in torch's layout
+        at the end, so that torch's own opt.step(closure) can take over. """
+        self._adopt_optimizer()
+        ev = self._eval_setup(niters, batch_size, sampler, loss_terms, criterion)
+        if ev is None:
+            return
+        entry_ids = {id(p) for p, _ in self.entries}
+        if any(id(p) not in entry_ids for p in opt.param_groups[0]['params']):
+            warnings.warn('pydens_b200: the optimizer holds parameters outside the fused network (a V() first met in a '
+                          'constraint that runs on autograd): torch.optim.LBFGS runs the update, over the fused '
+                          'evaluation', stacklevel=4)
+            self._fit_lbfgs_torch(niters, batch_size, sampler, ev, opt)
+            return
+        cfg, cur, mask = self._lbfgs_bind(opt)
+        dist = ev['dist']
+        if dist is not None:
+            dist.barrier()
+        self.solver.model.train()
+        status = torch.zeros(1, dtype=torch.int32, device=self.device)
+        status_host = torch.zeros(1, dtype=torch.int32).pin_memory()
+        start, ring_len = self.steps_done, self.ring.numel()
+        vals = np.empty(niters, dtype=np.float32)
+        host = ev['cols_key'] is None
+        total, off = ev['total'], ev['point_offset']
+        drained = 0
+        for i in _progress(niters):
+            points = full = None
+            if host:                                     # one host batch per step, staged once
+                b = sampler.sample(batch_size)
+                b = b if isinstance(b, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(b, dtype=np.float32))
+                full = b.detach().to(self.device, torch.float32).reshape(batch_size, total).contiguous()
+                if dist is not None and ev['nums']:
+                    dist.broadcast(full, 0)
+                points = full[off:off + ev['local_n']]
+            while True:
+                self._evaluate(ev, points, full if ev['nums'] else None)
+                _native.check(self.lib.pinn_lbfgs_advance(
+                    C.byref(cfg), C.c_int64(self.n_params), C.c_void_p(self.flat.data_ptr()),
+                    C.c_void_p(self.out.data_ptr()), C.c_void_p(cur['state'].data_ptr()),
+                    C.c_void_p(status.data_ptr()), self._stream()))
+                status_host.copy_(status, non_blocking=True)
+                torch.cuda.current_stream(self.device).synchronize()
+                if int(status_host[0]) == _native.LBFGS_DONE:
+                    break
+            if i + 1 - drained >= ring_len:
+                vals[drained:i + 1] = ring_losses(self.ring, start, drained, i + 1)
+                drained = i + 1
+        torch.cuda.synchronize(self.device)
+        vals[drained:] = ring_losses(self.ring, start, drained, niters)
+        token = lbfgs_export(cur['state'], opt, cur['idx'], self.n_params, cur['m'])
+        cur['fresh'] = token
+        self._end_stepwise(vals, dist)
+
+    def _fit_lbfgs_torch(self, niters, batch_size, sampler, ev, opt):
+        """ torch.optim.LBFGS.step(closure) with the fused evaluation (_evaluate) as its closure, one batch per step:
+        for optimizers over parameters the device update does not hold. """
+        self._lbfgs = None                               # opt.state is torch's own from here on
+        dist, total, off = ev['dist'], ev['total'], ev['point_offset']
+        self.solver.model.train()
+        losses = []
+        for _ in _progress(niters):
+            points = full = None
+            if ev['cols_key'] is None:
+                b = sampler.sample(batch_size)
+                b = b if isinstance(b, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(b, dtype=np.float32))
+                full = b.detach().to(self.device, torch.float32).reshape(batch_size, total).contiguous()
+                if dist is not None and ev['nums']:
+                    dist.broadcast(full, 0)
+                points = full[off:off + ev['local_n']]
+
+            def closure():
+                self._evaluate(ev, points, full if ev['nums'] else None)
+                return self.out[self.n_params].clone()
+            losses.append(float(opt.step(closure)))
+            self.step_counter += 1                       # the next step's batch
+        self.steps_done += niters
+        self.solver.losses.extend(np.array(v, dtype=np.float32) for v in losses)
 
     def _loop_in_kernel_sampler(self, niters, one_step, graphs_ok, opt_ready, key):
         """ Points sampled in the kernel: replays of a graph of `per_graph` steps, the rest as plain launches.
@@ -855,6 +995,77 @@ class FusedEngine:
                 raise RuntimeError('pydens_b200: a rank did not reach the in-kernel all-reduce within the time limit '
                                    '(PINN_COMM_TIMEOUT_S); the gradients of this fit were poisoned with NaN')
         self.solver.losses.extend(np.array(v, dtype=np.float32) for v in vals)
+
+
+def _lbfgs_views(state, n_params, m):
+    """ (header, fp64 arrays by name, vector slot accessor) of an L-BFGS state buffer (a uint8 device tensor) """
+    lay = _native.lbfgs_layout(n_params, m)
+    f64 = {k: state[o:o + 8 * c].view(torch.float64) for k, (o, c) in lay['f64'].items()}
+    nv = lay['nv']
+    vec = state[lay['vectors']:lay['total']].view(torch.float32)
+    return lay, f64, (lambda k: vec[k * nv:(k + 1) * nv])
+
+
+def lbfgs_import(state, st, idx, n_params, m):
+    """ torch.optim.LBFGS's state (`st`, the dict on its first parameter; vectors in the optimizer's parameter order)
+    into a zeroed device state: d, prev_flat_grad, the history pairs (oldest in slot 0) and their Gram entries, t,
+    H_diag, n_iter, func_evals, prev_loss. """
+    lay, f64, vec = _lbfgs_views(state, n_params, m)
+    S = lay['S']
+    hdr = _native.PinnLbfgsState()
+    hdr.n_iter, hdr.func_evals = int(st.get('n_iter', 0)), int(st.get('func_evals', 0))
+    hdr.t = float(st['t']) if st.get('t') is not None else 0.0
+    hdr.H_diag = float(st['H_diag']) if st.get('H_diag') is not None else 1.0
+    hdr.prev_loss = float(st['prev_loss']) if st.get('prev_loss') is not None else 0.0
+
+    def put(k, v):
+        if v is not None:
+            vec(k)[idx] = v.detach().reshape(-1).to(torch.float32)
+    put(_native.LBFGS_D, st.get('d'))
+    put(_native.LBFGS_PG, st.get('prev_flat_grad'))
+    dirs, stps = list(st.get('old_dirs') or []), list(st.get('old_stps') or [])
+    k = len(dirs)
+    for i in range(k):
+        put(_native.LBFGS_RING + i, stps[i])
+        put(_native.LBFGS_RING + S + i, dirs[i])
+    if k:
+        s_ = torch.stack([vec(_native.LBFGS_RING + i) for i in range(k)]).double()
+        y_ = torch.stack([vec(_native.LBFGS_RING + S + i) for i in range(k)]).double()
+        sy = f64['sy'].view(S, S)
+        yy = f64['yy'].view(S, S)
+        sy[:k, :k] = s_ @ y_.T
+        yy[:k, :k] = y_ @ y_.T
+    hdr.ring_count, hdr.ring_head = k, 0
+    state[:C.sizeof(hdr)].copy_(torch.frombuffer(bytearray(bytes(hdr)), dtype=torch.uint8))
+
+
+def lbfgs_export(state, opt, idx, n_params, m):
+    """ The device state into opt.state in torch.optim.LBFGS's layout (vectors gathered in the optimizer's parameter
+    order).  -> a predicate telling whether opt.state still holds exactly this write-back (torch has not stepped). """
+    lay, f64, vec = _lbfgs_views(state, n_params, m)
+    S = lay['S']
+    hdr = _native.PinnLbfgsState.from_buffer_copy(bytes(state[:C.sizeof(_native.PinnLbfgsState)].cpu().numpy()))
+    p0 = opt.param_groups[0]['params'][0]
+    st = opt.state[p0]
+    st['n_iter'], st['func_evals'] = int(hdr.n_iter), int(hdr.func_evals)
+    if hdr.n_iter == 0:
+        return lambda o: o.state.get(p0) is st and st.get('n_iter') == 0
+    k, head = int(hdr.ring_count), int(hdr.ring_head)
+    slots = [(head + i) % S for i in range(k)]
+    sy = f64['sy'].view(S, S)
+    st['d'] = vec(_native.LBFGS_D)[idx].clone()
+    st['t'] = float(hdr.t)
+    st['old_stps'] = [vec(_native.LBFGS_RING + p)[idx].clone() for p in slots]
+    st['old_dirs'] = [vec(_native.LBFGS_RING + S + p)[idx].clone() for p in slots]
+    st['ro'] = [(1.0 / sy[p, p]).float() for p in slots]
+    st['H_diag'] = torch.tensor(float(hdr.H_diag), dtype=torch.float32, device=state.device)
+    st['prev_flat_grad'] = vec(_native.LBFGS_PG)[idx].clone()
+    st['prev_loss'] = float(hdr.prev_loss)
+    al = f64['al'][:k].float()
+    st['al'] = [al[i] for i in range(k)] + [None] * (int(opt.param_groups[0]['history_size']) - k)
+    d = st['d']
+    n_iter = st['n_iter']
+    return lambda o: o.state.get(p0) is st and st.get('d') is d and st.get('n_iter') == n_iter
 
 
 class _RawPtr:

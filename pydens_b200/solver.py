@@ -298,7 +298,12 @@ class Solver:
         loss_terms  'equation' and/or 'constraint_{k}' (reference :382-389).  A constraint that evaluates the model once
                     at fixed points, optionally differentiated along them (`D(u(t0), t0)` with t0 requiring grad), and
                     combines the result pointwise runs as a fused launch on its points; any other is added by autograd.
-        optimizer   name from torch.optim; None re-uses the existing optimizer (reference :391-393).
+        optimizer   name from torch.optim; None re-uses the existing optimizer (reference :391-393).  'LBFGS' takes the
+                    torch.optim.LBFGS arguments as kwargs (max_iter, max_eval, tolerance_grad, tolerance_change,
+                    history_size, line_search_fn=None or 'strong_wolfe') and usually wants lr=1 (torch's default), not
+                    fit's 0.005.  One iteration is one `optimizer.step(closure)`: every evaluation within it sees that
+                    iteration's batch, and `losses` gets the loss of its first evaluation.  On the fused path the
+                    L-BFGS update itself runs on the device, one kernel per evaluation (pinn_lbfgs_advance).
         criterion   nn.MSELoss() (default), nn.L1Loss(), nn.HuberLoss(delta), nn.SmoothL1Loss(beta), mean or sum reduction,
                     train on the fused kernels (switching the criterion between fits rebuilds the engine); anything
                     else runs on the autograd path.
@@ -372,19 +377,26 @@ class Solver:
         self._make_optimizer(optimizer, lr, **kwargs)
         nums = self._constraint_numbers(loss_terms)
         self.model.train()
+        closure_opt = isinstance(self.optimizer, torch.optim.LBFGS)
         for _ in _progress(niters):
-            self.optimizer.zero_grad()
             xs = self._sample_host(sampler, batch_size)
-            for x in xs:
-                x.requires_grad_()
-            u_hat = self.ctx.run(self.model, self.reshape_and_concat(xs))
-            loss = 0
-            if 'equation' in loss_terms:
-                loss = loss + criterion(self.ctx.run(self.equation, u_hat, *xs), torch.zeros_like(xs[0]))
-            if nums:
-                loss = loss + self._constraint_loss(nums, xs, criterion)
-            loss.backward()
-            self.optimizer.step()
+
+            def closure():
+                self.optimizer.zero_grad()
+                pts = [x.detach().requires_grad_() for x in xs]
+                u_hat = self.ctx.run(self.model, self.reshape_and_concat(pts))
+                loss = 0
+                if 'equation' in loss_terms:
+                    loss = loss + criterion(self.ctx.run(self.equation, u_hat, *pts), torch.zeros_like(pts[0]))
+                if nums:
+                    loss = loss + self._constraint_loss(nums, pts, criterion)
+                loss.backward()
+                return loss
+            if closure_opt:                      # L-BFGS evaluates the batch as often as its step needs
+                loss = self.optimizer.step(closure)
+            else:
+                loss = closure()
+                self.optimizer.step()
             self.losses.append(loss.detach().cpu().numpy())
 
     def _release_engine(self):
