@@ -566,6 +566,44 @@ size_t pinn_lbfgs_vector_offset(int history_size);
 int pinn_lbfgs_advance(const PinnLbfgs* cfg, int64_t n_params, float* params, const float* grads_and_loss,
                        void* state, int* status, void* stream);
 
+/*
+ * L-BFGS IN THE PERSISTENT CLUSTER KERNEL: `n_steps` whole L-BFGS steps of a tiny-batch fit in one launch, with no
+ * launch and no host synchronisation between the evaluations of a step.  Each evaluation is the objective of
+ * pinn_multi_step_terms (the batch at point_weight, plus the constraint terms) at the current parameters; cluster rank 0
+ * then runs the state machine of pinn_lbfgs_advance on its shared-memory copy of the parameters, and the other CTAs of
+ * the cluster copy the parameters it asks to evaluate.  A step draws its batch once, at the step number *step_counter
+ * has when it begins (or reads points[s], s = 0 .. n_steps-1, [n_steps, n_points, ndims+nparams] on the device), and
+ * keeps it for all of its evaluations; when the step is done the state machine logs its first loss and advances the
+ * counter, exactly as pinn_lbfgs_advance does.  The state buffer has the layout of pinn_lbfgs_advance, so the two calls
+ * continue each other's state.  cfg->mask, losses_ring (not NULL here) and step_counter are the fit's, cfg->lr its step
+ * size.  Stream-ordered, capturable, allocates nothing.
+ *   plans without the cluster kernel (PinnPlanInfo.small_batch_points == 0): PINN_E_UNSUPPORTED;
+ *   a null pointer, n_steps < 1, n_points + constraint points outside 1 .. small_batch_points, settings
+ *   pinn_lbfgs_advance refuses, and what pinn_multi_step_terms refuses in the terms: PINN_E_INVALID.
+ * The cluster size is that of pinn_multi_step_terms for the same columns (PINN_SMALL_CLUSTER overrides).
+ *
+ * pinn_lbfgs_multi_ensemble: the same for n_members (1 .. PINN_MAX_MEMBERS) fits of one plan side by side, one cluster
+ * each.  A PinnLbfgsMember holds what differs between them; cfg's lr, mask, losses_ring and step_counter are not read,
+ * every other setting (and the terms, batch size, point weight, columns) is shared.  The members share nothing at run
+ * time: each one's result is bit-identical to pinn_lbfgs_multi on it alone.
+ */
+typedef struct PinnLbfgsMember {
+    float* params;             /* device [n_params] in/out, 16-byte aligned */
+    void* state;               /* device L-BFGS state buffer (pinn_lbfgs_state_bytes) in/out */
+    const float* mask;         /* device [n_params]: 1 = in the optimizer */
+    const float* points;       /* device [n_steps, n_points, ndims+nparams], or NULL: sample in-kernel */
+    uint64_t seed;
+    uint64_t* step_counter;    /* device step number of the member, += n_steps */
+    float* losses_ring;        /* device [cfg->ring_len] */
+    double lr;
+} PinnLbfgsMember;
+int pinn_lbfgs_multi(const PinnPlan* plan, const PinnLbfgs* cfg, float* params, void* state, const float* points,
+                     const PinnColumn* cols, uint64_t seed, int64_t n_points, int n_steps, float point_weight,
+                     int n_terms, const PinnTerm* terms, void* stream);
+int pinn_lbfgs_multi_ensemble(const PinnPlan* plan, const PinnLbfgs* cfg, int n_members, const PinnLbfgsMember* members,
+                              const PinnColumn* cols, int64_t n_points, int n_steps, float point_weight, int n_terms,
+                              const PinnTerm* terms, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -129,6 +129,12 @@ class PinnLbfgsState(C.Structure):
                 ('r_dot', C.c_double), ('r_max', C.c_double), ('r_l1', C.c_double)]
 
 
+class PinnLbfgsMember(C.Structure):
+    """ One fit of pinn_lbfgs_multi_ensemble: its parameters, state buffer, mask, batches, seed, counter, ring and lr. """
+    _fields_ = [('params', C.c_void_p), ('state', C.c_void_p), ('mask', C.c_void_p), ('points', C.c_void_p),
+                ('seed', C.c_uint64), ('step_counter', C.c_void_p), ('losses_ring', C.c_void_p), ('lr', C.c_double)]
+
+
 LBFGS_HEADER_BYTES, LBFGS_DONE, LBFGS_EVALUATE = 512, 0, 1
 LBFGS_D, LBFGS_PG, LBFGS_X, LBFGS_RING = 0, 1, 2, 6        # vector slots of the state buffer
 
@@ -153,7 +159,8 @@ EXPORTS = ('pinn_last_error', 'pinn_abi_version', 'pinn_plan_create', 'pinn_plan
            'pinn_step_allreduce', 'pinn_comm_status', 'pinn_pipe_create', 'pinn_pipe_destroy', 'pinn_pipe_buffer',
            'pinn_pipe_step', 'pinn_pipe_finish', 'pinn_pipe_wait', 'pinn_pipe_sync', 'pinn_multi_step',
            'pinn_multi_step_max_points', 'pinn_step_adam', 'pinn_multi_step_terms', 'pinn_multi_step_ensemble',
-           'pinn_multi_step_ensemble_adam', 'pinn_lbfgs_state_bytes', 'pinn_lbfgs_vector_offset', 'pinn_lbfgs_advance')
+           'pinn_multi_step_ensemble_adam', 'pinn_lbfgs_state_bytes', 'pinn_lbfgs_vector_offset', 'pinn_lbfgs_advance',
+           'pinn_lbfgs_multi', 'pinn_lbfgs_multi_ensemble')
 
 LIB_PATH = os.environ.get('PYDENS_B200_LIB') or os.path.join(os.path.dirname(os.path.abspath(__file__)), 'libpinn_b200.so')
 _lib = None
@@ -233,6 +240,12 @@ def load():
     lib.pinn_lbfgs_vector_offset.argtypes = [C.c_int]
     lib.pinn_lbfgs_advance.argtypes = [C.POINTER(PinnLbfgs), C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p]
+    lib.pinn_lbfgs_multi.argtypes = [C.c_void_p, C.POINTER(PinnLbfgs), C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.POINTER(PinnColumn), C.c_uint64, C.c_int64, C.c_int, C.c_float, C.c_int,
+                                     C.POINTER(PinnTerm), C.c_void_p]
+    lib.pinn_lbfgs_multi_ensemble.argtypes = [C.c_void_p, C.POINTER(PinnLbfgs), C.c_int, C.POINTER(PinnLbfgsMember),
+                                              C.POINTER(PinnColumn), C.c_int64, C.c_int, C.c_float, C.c_int,
+                                              C.POINTER(PinnTerm), C.c_void_p]
     if lib.pinn_abi_version() != ABI_VERSION:
         raise LibraryMissing('libpinn_b200.so ABI %d != binding ABI %d: rebuild' % (lib.pinn_abi_version(), ABI_VERSION))
     _lib = lib

@@ -9,7 +9,7 @@
 #define PINN_STEP_GMEM 3     // five / six directions: the general step_kernel with per-point state in global memory
 #define PINN_HI_JET 4        // hi_step_kernel, derivatives of order 3 / 4
 #define PINN_WIDE 5          // wide_step_kernel, the tensor-core tile kernel
-#define PINN_SMALL 6         // small_step_kernel, the tiny-batch cluster kernel (both forms)
+#define PINN_SMALL 6         // small_step_kernel, the tiny-batch cluster kernel (both Adam forms and the L-BFGS form)
 #define PINN_WIDE128 7       // wide_step_kernel of the 128-wide class
 #define PINN_COUPLED 8       // coupled_step_kernel, networks of 2..4 outputs
 #define PINN_WIDE128_COUPLED 9   // wide128_coupled_step_kernel, networks of 2..4 outputs on the 128-wide class
@@ -19,7 +19,7 @@
 #elif PINN_UNIT == PINN_WIDE || PINN_UNIT == PINN_WIDE128 || PINN_UNIT == PINN_WIDE128_COUPLED
 #include "pinn_wide_kernel.cuh"
 #elif PINN_UNIT == PINN_SMALL
-#include "pinn_small_kernel.cuh"
+#include "pinn_small_lbfgs.cuh"
 #else
 #include "pinn_step_kernel.cuh"
 #endif
@@ -63,6 +63,7 @@ void enter() {
 #elif PINN_UNIT == PINN_SMALL
     kernel_slot(NF, J, 2).small = small::small_step_kernel<NF, J>;
     kernel_slot(NF, J, 2).small_ensemble = small::small_step_ensemble_kernel<NF, J>;
+    kernel_slot(NF, J, 2).small_lbfgs = small::small_lbfgs_kernel<NF, J>;
 #elif PINN_UNIT == PINN_COUPLED
     using Cfg = VariantCfg<NF, J>;
     KernelSet& k = kernel_slot(NF, J, 2);

@@ -23,6 +23,7 @@
 #include "pinn_step_kernel.cuh"
 #include "pinn_wide_kernel.cuh"
 #include "pinn_small_kernel.cuh"
+#include "pinn_lbfgs.cuh"
 #include "pinn_host_plan.h"
 
 namespace pinn {
@@ -188,6 +189,13 @@ struct PersistentLaunch {
     int threads, smem, budget;
 };
 
+// The L-BFGS form of the cluster kernel (pinn_lbfgs_multi): null where the cluster kernel is, or where its static shared
+// memory leaves no room for the cluster kernel's layout.
+struct LbfgsLaunch {
+    LbfgsKernelFn fn;
+    int threads, smem, budget;
+};
+
 struct PinnPlan {
     PinnSpec spec;
     DevPlan h;
@@ -200,6 +208,7 @@ struct PinnPlan {
     StepLaunch step;
     ForwardLaunch fwd;
     PersistentLaunch multi, small;
+    LbfgsLaunch small_lbfgs;
 };
 
 extern "C" const char* pinn_last_error(void) { return g_err; }
@@ -354,6 +363,18 @@ static PersistentLaunch place_persistent(const PinnPlan* p, MultiKernelFn f, Ens
     return k;
 }
 
+// The L-BFGS form of the cluster kernel, where it runs NT threads in the `smem` bytes of the cluster kernel's layout.
+static LbfgsLaunch place_lbfgs(const PinnPlan* p, LbfgsKernelFn f, int smem) {
+    LbfgsLaunch k = {};
+    cudaFuncAttributes fa;
+    int budget;
+    if (kernel_budget((const void*)f, p->smem_optin, fa, budget) == cudaSuccess && max_warps(fa, small::NT) * 32 >= small::NT &&
+        smem <= budget && allow_max_smem((const void*)f, p->smem_optin) == cudaSuccess)
+        k = {f, small::NT, smem, budget};
+    (void)cudaGetLastError();
+    return k;
+}
+
 // Wide networks: the tensor-core tile kernel takes the step (PINN_FORCE_KERNEL=thread|wide|wide128 overrides).
 // thread_rc is how the thread kernel's placement (step and forward) went: a network whose weights do not fit its
 // shared memory goes to the 128-wide class when that class covers it; otherwise that failure is the plan's.
@@ -469,6 +490,7 @@ extern "C" int pinn_plan_create(const PinnSpec* s, int device, PinnPlan** out) {
         if (chain)
             p->small = place_persistent(p.get(), p->ks->small, p->ks->small_ensemble, small::NT,
                                         [&](int) { return small::make_layout(h).total * 4; });
+        if (p->small.solo && p->ks->small_lbfgs) p->small_lbfgs = place_lbfgs(p.get(), p->ks->small_lbfgs, p->small.smem);
     }
     if (int rc = place_tile_step(p.get(), order, thread_rc, tile)) return rc;
     p->step = tile.fn ? tile : thread;
@@ -814,8 +836,9 @@ struct MultiLaunch {
     int nc, smem;
 };
 
+// cluster_only: the cluster kernel whatever the batch (pinn_lbfgs_multi), for at most 8 x small::BP columns.
 static int multi_setup(PinnPlan* p, int64_t n_points, int k_steps, int64_t ring_len, float point_weight, int n_terms,
-                       const PinnTerm* terms, MultiLaunch& L) {
+                       const PinnTerm* terms, MultiLaunch& L, bool cluster_only = false) {
     if (!p->multi.solo && !p->small.solo) return fail(PINN_E_UNSUPPORTED, "the persistent multi-step kernels do not fit this network in shared memory");
     if (n_terms < 0 || n_terms > PINN_MAX_TERMS || (n_terms > 0 && !terms))
         return fail(PINN_E_INVALID, "pinn_multi_step_terms: %d terms (0..%d)", n_terms, PINN_MAX_TERMS);
@@ -842,9 +865,10 @@ static int multi_setup(PinnPlan* p, int64_t n_points, int k_steps, int64_t ring_
     }
     a.terms.first[n_terms] = a.terms.n_points;
     const long long n_cols = n_points + a.terms.n_points;
-    if (n_points <= 0 || n_cols > pinn_multi_step_max_points(p) || k_steps <= 0 || ring_len <= 0)
+    const int max_cols = cluster_only ? 8 * pinn::small::BP : pinn_multi_step_max_points(p);
+    if (n_points <= 0 || n_cols > max_cols || k_steps <= 0 || ring_len <= 0)
         return fail(PINN_E_INVALID, "pinn_multi_step: n_points %lld + %d constraint points (1..%d), k_steps %d", (long long)n_points,
-                    a.terms.n_points, pinn_multi_step_max_points(p), k_steps);
+                    a.terms.n_points, max_cols, k_steps);
     L.plan = p->h;
     L.plan.n_slots = n_slots;                                       // the small kernel's scratch rows
     a.n_points = n_points; a.inv_n = point_weight; a.k_steps = k_steps;
@@ -852,8 +876,8 @@ static int multi_setup(PinnPlan* p, int64_t n_points, int k_steps, int64_t ring_
     a.rows_total = rows;
     // batches of at most 128 points: the (point, unit)-parallel kernel (PINN_MULTI_KERNEL=tile forces the other one)
     const char* mk = getenv("PINN_MULTI_KERNEL");
-    const bool small = p->small.solo && n_cols <= 8 * pinn::small::BP && (n_cols <= 256 || !p->multi.solo) &&
-                       !(mk && !strcmp(mk, "tile") && p->multi.solo);
+    const bool small = cluster_only || (p->small.solo && n_cols <= 8 * pinn::small::BP && (n_cols <= 256 || !p->multi.solo) &&
+                                        !(mk && !strcmp(mk, "tile") && p->multi.solo));
     L.k = small ? &p->small : &p->multi;
     if (small) L.smem = n_slots == p->h.n_slots ? L.k->smem : small::make_layout(L.plan).total * 4;
     else       L.smem = rows == p->h.rows_total ? L.k->smem : multi_smem_bytes(p->h, L.k->threads / 32, rows);
@@ -985,6 +1009,61 @@ extern "C" int pinn_multi_step(const PinnPlan* p, float* params, float* exp_avg,
     return pinn_multi_step_terms(p, params, exp_avg, exp_avg_sq, mask, step_tensors, n_step_tensors, points, cols, seed,
                                  step_counter, n_points, k_steps, lr, beta1, beta2, eps, weight_decay, opt_step0,
                                  losses_ring, ring_len, n_points > 0 ? 1.0f / (float)n_points : 0.0f, 0, nullptr, stream);
+}
+
+// The launch of both L-BFGS entry points: cfg's shared settings as pinn_lbfgs_advance checks them, each member's own
+// pointers and lr, then the columns as pinn_multi_step_terms checks them, on the cluster kernel only.
+static int lbfgs_multi(const PinnPlan* cp, const PinnLbfgs* cfg, int n_members, const PinnLbfgsMember* members,
+                       const PinnColumn* cols, int64_t n_points, int n_steps, float point_weight, int n_terms,
+                       const PinnTerm* terms, void* stream) {
+    PinnPlan* p = const_cast<PinnPlan*>(cp);
+    if (!p || !cfg || !members) return fail(PINN_E_INVALID, "pinn_lbfgs_multi: null argument");
+    if (!p->small_lbfgs.fn)
+        return fail(PINN_E_UNSUPPORTED, "pinn_lbfgs_multi: the cluster kernel does not fit this network (small_batch_points = 0)");
+    if (cfg->max_iter < 1 || cfg->max_eval < 1 || cfg->history_size < 1 || (cfg->line_search != 0 && cfg->line_search != 1) ||
+        cfg->ring_len < 1)
+        return fail(PINN_E_INVALID, "pinn_lbfgs_multi: invalid settings (max_iter %d, max_eval %d, history_size %d, line_search %d, "
+                    "ring_len %lld)", cfg->max_iter, cfg->max_eval, cfg->history_size, cfg->line_search, (long long)cfg->ring_len);
+    if (n_members < 1 || n_members > PINN_MAX_MEMBERS)
+        return fail(PINN_E_INVALID, "pinn_lbfgs_multi_ensemble: %d members (1..%d)", n_members, PINN_MAX_MEMBERS);
+    bool sample = false;
+    for (int j = 0; j < n_members; ++j) {
+        const PinnLbfgsMember& m = members[j];
+        if (!m.params || !m.state || !m.mask || !m.step_counter || !m.losses_ring)
+            return fail(PINN_E_INVALID, "pinn_lbfgs_multi: member %d: null pointer", j);
+        if (!aligned16(m.params) || !aligned16(m.state))
+            return fail(PINN_E_INVALID, "pinn_lbfgs_multi: member %d: params and state must be 16-byte aligned", j);
+        if (!(m.lr >= 0.0)) return fail(PINN_E_INVALID, "pinn_lbfgs_multi: member %d: lr %g", j, m.lr);
+        if (!m.points) sample = true;
+    }
+    if (n_steps < 1) return fail(PINN_E_INVALID, "pinn_lbfgs_multi: n_steps %d", n_steps);
+    static thread_local MultiLaunch L;                               // 13 KB: off the stack
+    static thread_local DevLbfgsMembers table;                       // 8 KB
+    if (int rc = multi_setup(p, n_points, n_steps, cfg->ring_len, point_weight, n_terms, terms, L, true))
+        return rc;
+    if (L.smem > p->small_lbfgs.budget)
+        return fail(PINN_E_UNSUPPORTED, "pinn_lbfgs_multi: the constraint programs' scratch slots do not fit shared memory");
+    if (sample) { int rc = resolve_cols(p, cols, L.plan.cols); if (rc) return rc; }
+    memset(&table, 0, sizeof(table));
+    table.cfg = *cfg;
+    memcpy(table.m, members, sizeof(PinnLbfgsMember) * (size_t)n_members);
+    return launch_persistent(p->small_lbfgs.fn, L, n_members, stream, table);
+}
+
+extern "C" int pinn_lbfgs_multi(const PinnPlan* plan, const PinnLbfgs* cfg, float* params, void* state, const float* points,
+                                const PinnColumn* cols, uint64_t seed, int64_t n_points, int n_steps, float point_weight,
+                                int n_terms, const PinnTerm* terms, void* stream) {
+    if (!cfg) return fail(PINN_E_INVALID, "pinn_lbfgs_multi: null argument");
+    PinnLbfgsMember m;
+    m.params = params; m.state = state; m.mask = cfg->mask; m.points = points; m.seed = seed;
+    m.step_counter = cfg->step_counter; m.losses_ring = cfg->losses_ring; m.lr = cfg->lr;
+    return lbfgs_multi(plan, cfg, 1, &m, cols, n_points, n_steps, point_weight, n_terms, terms, stream);
+}
+
+extern "C" int pinn_lbfgs_multi_ensemble(const PinnPlan* plan, const PinnLbfgs* cfg, int n_members,
+                                         const PinnLbfgsMember* members, const PinnColumn* cols, int64_t n_points,
+                                         int n_steps, float point_weight, int n_terms, const PinnTerm* terms, void* stream) {
+    return lbfgs_multi(plan, cfg, n_members, members, cols, n_points, n_steps, point_weight, n_terms, terms, stream);
 }
 
 extern "C" int pinn_forward(const PinnPlan* p, const float* params, const float* points, int64_t n_points,

@@ -15,40 +15,6 @@ namespace lbfgs {
 static const int THREADS = 512;
 static const int STAGE_MAX_BYTES = 192 * 1024;
 
-// Reductions of the CTA in a fixed order: lanes by a shuffle tree into lane 0, warps by thread 0 in warp order.
-struct CtaExec {
-    int tid, nt, lane, nl, warp, nw;
-    double* red;                                      // shared [2 * nw]
-    __device__ CtaExec(double* red_) : red(red_) {
-        tid = threadIdx.x; nt = blockDim.x; lane = tid & 31; nl = 32; warp = tid >> 5; nw = nt >> 5;
-    }
-    __device__ double wsum(double v) {
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-        return __shfl_sync(0xffffffffu, v, 0);
-    }
-    __device__ double wmax(double v) {
-        for (int o = 16; o > 0; o >>= 1) v = nan_max(v, __shfl_down_sync(0xffffffffu, v, o));
-        return __shfl_sync(0xffffffffu, v, 0);
-    }
-    __device__ double block(double v, bool is_max) {
-        v = is_max ? wmax(v) : wsum(v);
-        __syncthreads();
-        if (lane == 0) red[warp] = v;
-        __syncthreads();
-        if (tid == 0) {
-            double a = red[0];
-            for (int w = 1; w < nw; ++w) a = is_max ? nan_max(a, red[w]) : a + red[w];
-            red[nw] = a;
-        }
-        __syncthreads();
-        return red[nw];
-    }
-    __device__ double bsum(double v) { return block(v, false); }
-    __device__ double bmax(double v) { return block(v, true); }
-    __device__ void bsync() { __syncthreads(); }
-    __device__ void wsync() { __syncwarp(); }
-};
-
 __global__ void __launch_bounds__(THREADS, 1)
 lbfgs_advance_kernel(const PinnLbfgs c, int64_t n, float* params, const float* out, void* state, int* status,
                      int stage_on) {

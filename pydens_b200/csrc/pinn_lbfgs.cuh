@@ -273,7 +273,7 @@ LB_HD int lbfgs_control(const PinnLbfgs& c, PinnLbfgsState* h, const double* sy,
     }
 }
 
-// Where the vector passes run: a CTA (pinn_lbfgs.cu: CtaExec) or one host thread (HostExec below).  Exec provides tid /
+// Where the vector passes run: a CTA (CtaExec below) or one host thread (HostExec below).  Exec provides tid /
 // nt (thread and thread count), lane / nl / warp / nw, wsum (warp sum, the same value in every lane), bsum / bmax
 // (block reductions, the same value in every thread), bsync, wsync.
 
@@ -438,6 +438,42 @@ LB_HD void lbfgs_pass(E& ex, const PinnLbfgs& c, PinnLbfgsState* h, const View<T
         break;
     }
 }
+
+#if defined(__CUDACC__)
+// Reductions of the CTA in a fixed order: lanes by a shuffle tree into lane 0, warps by thread 0 in warp order.
+struct CtaExec {
+    int tid, nt, lane, nl, warp, nw;
+    double* red;                                      // shared [2 * nw]
+    __device__ CtaExec(double* red_) : red(red_) {
+        tid = threadIdx.x; nt = blockDim.x; lane = tid & 31; nl = 32; warp = tid >> 5; nw = nt >> 5;
+    }
+    __device__ double wsum(double v) {
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+        return __shfl_sync(0xffffffffu, v, 0);
+    }
+    __device__ double wmax(double v) {
+        for (int o = 16; o > 0; o >>= 1) v = nan_max(v, __shfl_down_sync(0xffffffffu, v, o));
+        return __shfl_sync(0xffffffffu, v, 0);
+    }
+    __device__ double block(double v, bool is_max) {
+        v = is_max ? wmax(v) : wsum(v);
+        __syncthreads();
+        if (lane == 0) red[warp] = v;
+        __syncthreads();
+        if (tid == 0) {
+            double a = red[0];
+            for (int w = 1; w < nw; ++w) a = is_max ? nan_max(a, red[w]) : a + red[w];
+            red[nw] = a;
+        }
+        __syncthreads();
+        return red[nw];
+    }
+    __device__ double bsum(double v) { return block(v, false); }
+    __device__ double bmax(double v) { return block(v, true); }
+    __device__ void bsync() { __syncthreads(); }
+    __device__ void wsync() { __syncwarp(); }
+};
+#endif
 
 #if !defined(__CUDACC__)
 struct HostExec {

@@ -583,6 +583,15 @@ struct DevMembers {
 // 13 344 + 12 800 = 26 144 bytes
 static_assert(sizeof(DevPlan) + sizeof(MultiArgs) + sizeof(DevMembers) + 32 <= 32764,
               "DevPlan + MultiArgs + the member table exceed the kernel-parameter limit");
+// The member table of the L-BFGS form of the cluster kernel (pinn_lbfgs_multi, pinn_lbfgs_multi_ensemble): the shared
+// settings, and what differs between the fits.  A solo fit is a table of one.
+struct DevLbfgsMembers {
+    PinnLbfgs cfg;
+    PinnLbfgsMember m[PINN_MAX_MEMBERS];
+};
+// 13 344 + 8 256 bytes
+static_assert(sizeof(DevPlan) + sizeof(MultiArgs) + sizeof(DevLbfgsMembers) + 32 <= 32764,
+              "DevPlan + MultiArgs + the L-BFGS member table exceed the kernel-parameter limit");
 
 // The body of both forms: the fields of `mb` (MultiArgs itself, or one row of the member table) are the fit's own state,
 // and those of `hy` (MultiArgs itself, or the member's row of hyper-parameters) its Adam hyper-parameters.
@@ -721,6 +730,7 @@ __global__ void __launch_bounds__(MAXT, 1) multi_step_ensemble_kernel(const __gr
 
 typedef void (*MultiKernelFn)(const DevPlan, const MultiArgs);
 typedef void (*EnsembleKernelFn)(const DevPlan, const MultiArgs, const DevMembers);
+typedef void (*LbfgsKernelFn)(const DevPlan, const MultiArgs, const DevLbfgsMembers);
 
 typedef void (*StepKernelFn)(const DevPlan, const StepArgs);
 
@@ -742,6 +752,7 @@ struct KernelSet {
     EnsembleKernelFn multi_ensemble;         // the ensemble forms of `multi` and `small` (null where those are)
     EnsembleKernelFn small_ensemble;
     StepKernelFn step_w12;                   // step_kernel_w12 (nf = ns = 2 only; null elsewhere)
+    LbfgsKernelFn small_lbfgs;               // the L-BFGS form of `small` (pinn_small_lbfgs.cuh; null where that is)
 };
 
 // The set of a jet set, or nullptr when none was built: 0 <= ns <= nf <= PINN_MAX_DIRS for order 2; 1 <= nf <= 4 and

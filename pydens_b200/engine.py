@@ -158,46 +158,30 @@ def ring_losses(ring, start, lo, hi):
     return ring.cpu().numpy()[(start + np.arange(lo, hi)) % ring.numel()]
 
 
-def run_persistent(engines, opts, samplers, terms, niters, batch_size, k, table):
-    """ `niters` optimizer steps of every engine's fit, `k` per launch of the persistent multi-step kernels: the
-    reference loop model_torch.py:426-464 with optimizer.step() inside the kernel, constraint terms included.  One fit
-    runs on the solo kernels (pinn_multi_step_terms) unless `table` is set; with `table` the fits are members of
-    pinn_multi_step_ensemble_adam, at most MAX_MEMBERS per launch, each with the Adam hyper-parameters of its own
-    optimizer.  `samplers` has one sampler per fit: all in-kernel with the same columns, or all on the host.  Returns
-    None, or the library's message when it refused the first launch with PINN_E_UNSUPPORTED (no step has been taken
-    then). """
-    e0 = engines[0]
-    lib, total, ring_len = e0.lib, e0.solver.model.total, e0.ring.numel()
-    # point weights: the mean of model_torch.py:448 over the batch and over every constraint's own points, or 1
-    total_sum = e0._sum_reduction()
+def _term_array(terms, total_sum):
+    """ The constraint terms of a persistent fit as a PinnTerm array, with their point weights: the mean of
+    model_torch.py:448 over every constraint's own points, or 1 for reduction='sum'. """
     term_arr = (_native.PinnTerm * max(1, len(terms)))()
     for i, e in enumerate(terms):
         term_arr[i].plan = e['plan'].value
         term_arr[i].n_points = e['n']
         term_arr[i].point_weight = 1.0 if total_sum else 1.0 / e['n']
         term_arr[i].points = e['host_points'].data_ptr()
-    point_weight = 1.0 if total_sum else 1.0 / batch_size
-    M = len(engines)
-    members = (_native.PinnMember * M)()
-    hyper = (_native.PinnAdamHyper * M)()
-    starts, step0 = [], []
-    for mb, hy, eng, opt in zip(members, hyper, engines, opts):
-        hy.lr, (hy.beta1, hy.beta2), hy.eps, hy.weight_decay = adam_hyper(opt)
-        eng._adopt_optimizer()
-        mask = eng._bind_adam_state(opt)
-        m, v, steps, _ = eng._adam_flat
-        mb.params, mb.exp_avg, mb.exp_avg_sq, mb.mask = eng.flat.data_ptr(), m.data_ptr(), v.data_ptr(), mask.data_ptr()
-        mb.step_tensors, mb.n_step_tensors = steps.data_ptr(), steps.numel()
-        mb.seed, mb.step_counter, mb.losses_ring = eng.seed, eng.step_counter.data_ptr(), eng.ring.data_ptr()
-        step0.append(float(steps.max().item()))
-        starts.append(eng.steps_done)
-        eng.solver.model.train()
-    cols_key, cols = sampler_columns(samplers[0], total)
-    host = cols_key is None
-    lr, (b1, b2), eps, wd = adam_hyper(opts[0])
-    stream = e0._stream()
-    size, hsize = C.sizeof(_native.PinnMember), C.sizeof(_native.PinnAdamHyper)
-    vals = np.empty((M, niters), dtype=np.float32)
+    return term_arr
+
+
+def _persistent_launches(engines, samplers, niters, batch_size, k, members, launch):
+    """ The launch loop of a persistent fit: `niters` steps of every engine's fit, at most `k` (and the loss ring's
+    length) per launch.  For host samplers each member's batches of a launch are staged on the device and set in its
+    row of `members` (a ctypes array whose rows have `points`); `launch(done, kk)` then issues the launches of steps
+    done .. done + kk - 1 and returns None, or the library's message when it refused the first launch with
+    PINN_E_UNSUPPORTED (no step has been taken then: returned as it is).  The losses of every step are read from the
+    device rings and appended to each solver's `losses`; `steps_done` advances. """
+    e0 = engines[0]
+    total, ring_len = e0.solver.model.total, e0.ring.numel()
+    host = sampler_columns(samplers[0], total)[0] is None
+    starts = [eng.steps_done for eng in engines]
+    vals = np.empty((len(engines), niters), dtype=np.float32)
 
     def drain(lo, hi):
         torch.cuda.synchronize(e0.device)
@@ -211,14 +195,68 @@ def run_persistent(engines, opts, samplers, terms, niters, batch_size, k, table)
             drain(drained, done)
             drained = done
         batches = []                                      # each member's kk batches, alive until the launch
-        for mb, smp, s0 in zip(members, samplers, step0):
-            if host:
+        if host:
+            for mb, smp in zip(members, samplers):
                 pinned = torch.empty((kk, batch_size, total), dtype=torch.float32).pin_memory()
                 for i in range(kk):
                     b = smp.sample(batch_size)
                     pinned[i].copy_(b if isinstance(b, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(b, dtype=np.float32)))
                 batches.append(pinned.to(e0.device, non_blocking=True))
                 mb.points = batches[-1].data_ptr()
+        refused = launch(done, kk)
+        if refused is not None:
+            return refused
+        done += kk
+    drain(drained, niters)
+    for j, eng in enumerate(engines):
+        eng.steps_done = starts[j] + niters
+        eng.solver.losses.extend(np.array(x, dtype=np.float32) for x in vals[j])
+    return None
+
+
+def _first_refusal(rc, lib, done, lo):
+    """ The library's message when it refused the first launch of a fit as unsupported, else None (raises on other
+    errors). """
+    if rc == _native.E_UNSUPPORTED and done == 0 and lo == 0:
+        return lib.pinn_last_error().decode('utf-8', 'replace')
+    _native.check(rc)
+    return None
+
+
+def run_persistent(engines, opts, samplers, terms, niters, batch_size, k, table):
+    """ `niters` optimizer steps of every engine's fit, `k` per launch of the persistent multi-step kernels: the
+    reference loop model_torch.py:426-464 with optimizer.step() inside the kernel, constraint terms included.  One fit
+    runs on the solo kernels (pinn_multi_step_terms) unless `table` is set; with `table` the fits are members of
+    pinn_multi_step_ensemble_adam, at most MAX_MEMBERS per launch, each with the Adam hyper-parameters of its own
+    optimizer.  `samplers` has one sampler per fit: all in-kernel with the same columns, or all on the host.  Returns
+    None, or the library's message when it refused the first launch with PINN_E_UNSUPPORTED (no step has been taken
+    then). """
+    e0 = engines[0]
+    lib, total, ring_len = e0.lib, e0.solver.model.total, e0.ring.numel()
+    total_sum = e0._sum_reduction()
+    term_arr = _term_array(terms, total_sum)
+    point_weight = 1.0 if total_sum else 1.0 / batch_size
+    M = len(engines)
+    members = (_native.PinnMember * M)()
+    hyper = (_native.PinnAdamHyper * M)()
+    step0 = []
+    for mb, hy, eng, opt in zip(members, hyper, engines, opts):
+        hy.lr, (hy.beta1, hy.beta2), hy.eps, hy.weight_decay = adam_hyper(opt)
+        eng._adopt_optimizer()
+        mask = eng._bind_adam_state(opt)
+        m, v, steps, _ = eng._adam_flat
+        mb.params, mb.exp_avg, mb.exp_avg_sq, mb.mask = eng.flat.data_ptr(), m.data_ptr(), v.data_ptr(), mask.data_ptr()
+        mb.step_tensors, mb.n_step_tensors = steps.data_ptr(), steps.numel()
+        mb.seed, mb.step_counter, mb.losses_ring = eng.seed, eng.step_counter.data_ptr(), eng.ring.data_ptr()
+        step0.append(float(steps.max().item()))
+        eng.solver.model.train()
+    cols = sampler_columns(samplers[0], total)[1]
+    lr, (b1, b2), eps, wd = adam_hyper(opts[0])
+    stream = e0._stream()
+    size, hsize = C.sizeof(_native.PinnMember), C.sizeof(_native.PinnAdamHyper)
+
+    def launch(done, kk):
+        for mb, s0 in zip(members, step0):
             mb.opt_step0 = s0 + done
         for lo in range(0, M, _native.MAX_MEMBERS):
             if table:
@@ -235,15 +273,64 @@ def run_persistent(engines, opts, samplers, terms, niters, batch_size, k, table)
                     mb.points, cols, mb.seed, mb.step_counter, C.c_int64(batch_size), C.c_int(kk), C.c_float(lr),
                     C.c_float(b1), C.c_float(b2), C.c_float(eps), C.c_float(wd), C.c_float(mb.opt_step0),
                     mb.losses_ring, C.c_int64(ring_len), C.c_float(point_weight), C.c_int(len(terms)), term_arr, stream)
-            if rc == _native.E_UNSUPPORTED and done == 0 and lo == 0:
-                return lib.pinn_last_error().decode('utf-8', 'replace')
-            _native.check(rc)
-        done += kk
-    drain(drained, niters)
-    for j, eng in enumerate(engines):
-        eng.steps_done = starts[j] + niters
-        eng.solver.losses.extend(np.array(x, dtype=np.float32) for x in vals[j])
-    return None
+            refused = _first_refusal(rc, lib, done, lo)
+            if refused is not None:
+                return refused
+        return None
+
+    return _persistent_launches(engines, samplers, niters, batch_size, k, members, launch)
+
+
+def run_lbfgs_persistent(engines, opts, samplers, terms, niters, batch_size, k, table):
+    """ `niters` L-BFGS steps of every engine's fit, `k` per launch of the L-BFGS form of the cluster kernel: every
+    evaluation of a step and the update between them run in the kernel, on the step's one batch, with the constraint
+    terms.  One fit runs through pinn_lbfgs_multi unless `table` is set; with `table` the fits are members of
+    pinn_lbfgs_multi_ensemble, at most MAX_MEMBERS per launch, each with its own lr and frozen mask and the other
+    settings of opts[0].  Each device state is bound as _fit_lbfgs binds it and written back into opt.state at the end.
+    Returns None, or the library's message when it refused the first launch with PINN_E_UNSUPPORTED (no step has been
+    taken then). """
+    e0 = engines[0]
+    lib, total = e0.lib, e0.solver.model.total
+    total_sum = e0._sum_reduction()
+    term_arr = _term_array(terms, total_sum)
+    point_weight = 1.0 if total_sum else 1.0 / batch_size
+    M = len(engines)
+    members = (_native.PinnLbfgsMember * M)()
+    binds = []
+    for mb, eng, opt in zip(members, engines, opts):
+        eng._adopt_optimizer()
+        cfg, cur, mask = eng._lbfgs_bind(opt)
+        binds.append((cfg, cur, mask))
+        mb.params, mb.state, mb.mask = eng.flat.data_ptr(), cur['state'].data_ptr(), mask.data_ptr()
+        mb.seed, mb.step_counter, mb.losses_ring, mb.lr = eng.seed, eng.step_counter.data_ptr(), eng.ring.data_ptr(), cfg.lr
+        eng.solver.model.train()
+    cfg = binds[0][0]
+    cols = sampler_columns(samplers[0], total)[1]
+    stream = e0._stream()
+    size = C.sizeof(_native.PinnLbfgsMember)
+
+    def launch(done, kk):
+        for lo in range(0, M, _native.MAX_MEMBERS):
+            if table:
+                rc = lib.pinn_lbfgs_multi_ensemble(
+                    e0.plan, C.byref(cfg), min(_native.MAX_MEMBERS, M - lo),
+                    C.cast(C.addressof(members) + lo * size, C.POINTER(_native.PinnLbfgsMember)), cols,
+                    C.c_int64(batch_size), C.c_int(kk), C.c_float(point_weight), C.c_int(len(terms)), term_arr, stream)
+            else:
+                mb = members[0]
+                rc = lib.pinn_lbfgs_multi(e0.plan, C.byref(cfg), mb.params, mb.state, mb.points, cols, mb.seed,
+                                          C.c_int64(batch_size), C.c_int(kk), C.c_float(point_weight),
+                                          C.c_int(len(terms)), term_arr, stream)
+            refused = _first_refusal(rc, lib, done, lo)
+            if refused is not None:
+                return refused
+        return None
+
+    refused = _persistent_launches(engines, samplers, niters, batch_size, k, members, launch)
+    if refused is None:
+        for eng, opt, (_, cur, _) in zip(engines, opts, binds):
+            cur['fresh'] = lbfgs_export(cur['state'], opt, cur['idx'], eng.n_params, cur['m'])
+    return refused
 
 
 class FusedEngine:
@@ -583,6 +670,25 @@ class FusedEngine:
             return None
         return entries
 
+    def _lbfgs_persistent_terms(self, niters, batch_size, loss_terms, opt, steps_per_launch):
+        """ The constraint terms of an L-BFGS fit that runs in the cluster kernel (run_lbfgs_persistent), or None when
+        it does not: a plan without the cluster kernel, several ranks, an optimizer over parameters outside the fused
+        network, constraints that do not all lower to persistent terms, a batch the kernel does not take, or a fit the
+        rule of auto_persistent does not send there without steps_per_launch. """
+        cap = int(self.info.small_batch_points)
+        if niters <= 0 or batch_size <= 0 or not cap or _dist() is not None:
+            return None
+        if steps_per_launch <= 0 and not auto_persistent(niters, batch_size, self.info):
+            return None
+        g = opt.param_groups[0]
+        entry_ids = {id(p) for p, _ in self.entries}
+        if any(id(p) not in entry_ids for p in g['params']) or g['line_search_fn'] not in (None, 'strong_wolfe'):
+            return None
+        terms = self._persistent_terms(loss_terms, batch_size)
+        if terms is None or batch_size + sum(e['n'] for e in terms) > cap:
+            return None
+        return terms
+
     def _fit_persistent(self, niters, batch_size, sampler, opt, k, terms=()):
         """ `niters` optimizer steps, `k` per launch of the solo persistent multi-step kernels (run_persistent).
         Returns False, having taken no step, when the kernels cannot hold the constraint programs' scratch slots. """
@@ -602,9 +708,18 @@ class FusedEngine:
         # keeps one launch per step).  An explicit steps_per_launch takes precedence.
         requested = steps_per_launch > 0
         if type(opt) is torch.optim.LBFGS and len(opt.param_groups) == 1:
+            # tiny batches: every evaluation and update of a step in the L-BFGS form of the cluster kernel, by the same
+            # rule as Adam's persistent fits
+            terms = self._lbfgs_persistent_terms(niters, batch_size, loss_terms, opt, steps_per_launch)
+            k = steps_per_launch if requested else _AUTO_PERSISTENT_STEPS
+            if terms is not None and run_lbfgs_persistent([self], [opt], [sampler], terms, niters, batch_size, k,
+                                                          table=False) is None:
+                return
             if requested:
-                warnings.warn('pydens_b200: steps_per_launch ignored (L-BFGS runs one evaluation per launch)',
-                              stacklevel=3)
+                warnings.warn('pydens_b200: steps_per_launch ignored (L-BFGS runs in the cluster kernel only on one '
+                              'device, with fused constraints, over parameters of the fused network, for a batch of at '
+                              'most %d points with the constraint points; otherwise one evaluation per launch)'
+                              % int(self.info.small_batch_points), stacklevel=3)
             self._fit_lbfgs(niters, batch_size, sampler, loss_terms, criterion, opt)
             return
         if not requested and auto_persistent(niters, batch_size, self.info):

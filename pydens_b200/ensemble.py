@@ -6,16 +6,18 @@ cluster of at most 8 CTAs; `fit_ensemble` puts up to PINN_MAX_MEMBERS of them in
 (pinn_multi_step_ensemble), one CTA or cluster per member.  It means exactly "call `s.fit(...)` on every solver": every
 member keeps its own seed, optimizer state, frozen mask, loss list and step counter, and its result is bit-identical to
 its solo fit.  Each member may also take its own Adam hyper-parameters (a learning-rate sweep: `lr=[...]`), which the
-kernels read from the member's row of the table (pinn_multi_step_ensemble_adam).
+kernels read from the member's row of the table (pinn_multi_step_ensemble_adam).  L-BFGS fits whose solo fits run in
+the cluster kernel go to its L-BFGS form the same way (pinn_lbfgs_multi_ensemble), each with its own lr.
 """
 import warnings
 
 import numpy as np
+import torch
 from torch import nn
 
 from . import _native
-from .engine import (_AUTO_PERSISTENT_STEPS, _dist, adam_steps_equal, auto_persistent, plain_adam, run_persistent,
-                     sampler_columns)
+from .engine import (_AUTO_PERSISTENT_STEPS, _dist, adam_steps_equal, auto_persistent, plain_adam, run_lbfgs_persistent,
+                     run_persistent, sampler_columns)
 
 # what each part of the problem's spec describes, for the error that names the difference between two members
 _SPEC_PARTS = (
@@ -88,7 +90,8 @@ def fit_ensemble(solvers, niters, batch_size, sampler=None, loss_terms='equation
     """ `s.fit(niters, batch_size, sampler, loss_terms, optimizer, criterion, lr, ...)` for every solver in `solvers`,
     in one persistent launch per `steps_per_launch` steps for all of them when each fit is one that `Solver.fit` sends
     to the persistent multi-step kernels by itself (or with steps_per_launch): plain Adam, one device, the equation
-    term, fused constraints, a batch the kernels take.  The solvers must share the problem byte for byte (equation,
+    term, fused constraints, a batch the kernels take.  L-BFGS fits (optimizer='LBFGS') run together in the L-BFGS form
+    of the cluster kernel when each member's solo fit runs there and the members share every setting but lr.  The solvers must share the problem byte for byte (equation,
     network, domain, ansatz, constraints); they differ in their parameters, seeds, optimizer states and frozen masks.
 
     sampler   None, one sampler shared by all members, or a list with one per member.  In-kernel samplers draw each
@@ -164,14 +167,33 @@ def _fit_together(solvers, niters, batch_size, samplers, loss_terms, optimizer, 
     total = solvers[0].model.total
     if len({sampler_columns(smp, total)[0] for smp in samplers}) > 1:
         return 'the members\' samplers differ in their in-kernel columns, or some sample on the host'
-    opts = []
-    for eng, lr_j, kw in zip(engines, *member_hyper(len(solvers), lr, kwargs)):
-        opt, _ = eng._optimizer_for(optimizer, lr_j, kw)
+    opts = [eng._optimizer_for(optimizer, lr_j, kw)[0]
+            for eng, lr_j, kw in zip(engines, *member_hyper(len(solvers), lr, kwargs))]
+    if all(type(opt) is torch.optim.LBFGS and len(opt.param_groups) == 1 for opt in opts):
+        return _fit_lbfgs_together(engines, opts, samplers, loss_terms, niters, batch_size, k, int(steps_per_launch or 0))
+    for opt in opts:
         if not plain_adam(opt):
             return ('the optimizer is not plain torch.optim.Adam with one parameter group and L2 weight decay '
                     '(decoupled weight decay runs on torch\'s Adam)')
         if not adam_steps_equal(opt):
             return 'the optimizer has taken different numbers of steps for different parameters'
-        opts.append(opt)
     return run_persistent(engines, opts, samplers, terms[0], niters, batch_size, k, table=True)
+
+
+# the settings of torch.optim.LBFGS the members of one launch share (lr is each member's own)
+_LBFGS_SHARED = ('max_iter', 'max_eval', 'tolerance_grad', 'tolerance_change', 'history_size', 'line_search_fn')
+
+
+def _fit_lbfgs_together(engines, opts, samplers, loss_terms, niters, batch_size, k, steps_per_launch):
+    """ The L-BFGS ensemble fit in the L-BFGS form of the cluster kernel (run_lbfgs_persistent), when each member's
+    solo fit would run there, or the reason it cannot (nothing has been trained then). """
+    for j, (eng, opt) in enumerate(zip(engines, opts)):
+        if eng._lbfgs_persistent_terms(niters, batch_size, loss_terms, opt, steps_per_launch) is None:
+            return 'solver %d: its L-BFGS fit does not run in the cluster kernel' % j
+        g, g0 = opt.param_groups[0], opts[0].param_groups[0]
+        diff = [name for name in _LBFGS_SHARED if g[name] != g0[name]]
+        if diff:
+            return 'solver %d: its L-BFGS settings differ from solver 0\'s in %s' % (j, ', '.join(diff))
+    terms = engines[0]._persistent_terms(loss_terms, batch_size)
+    return run_lbfgs_persistent(engines, opts, samplers, terms, niters, batch_size, k, table=True)
 
